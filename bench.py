@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- molecules/sec of the 1000-step denoising sampler (BASELINE.json metric) on N B200s, one process per GPU.
+"""bench.py -- molecules/sec of the 1000-step denoising sampler (BASELINE.json metric) on N H100s, one process per GPU.
 
-    python bench.py --gpus 1 --steps K --warmup W            (driver contract; N>1 is launched through torchrun)
+    python bench.py --gpus 1 --steps K --warmup W            (N>1 is launched through torchrun)
+    python bench.py ... --dump-outputs DIR                    (also write the last timed step's outputs as DIR/<name>.npy)
     python bench.py --impl reference ...                      (the reference's algorithm on the host cores: CPU oracle port)
 
 What a "step" is: one pass of the hot path -- one denoising step (k-NN graph + 9 attention layers + type head +
@@ -34,7 +35,7 @@ WORKLOADS = {
     'cfg3': dict(pockets=64, samples=10, n_protein=300, n_ligand=20, knn=32),
     'cfg5': dict(pockets=64, samples=1, n_protein=1200, n_ligand=40, knn=48),
 }
-DTYPE = 'f32 (storage, LayerNorm, softmax, accumulation); GEMM operands as 2-piece bf16 splits on tcgen05 (3 products, ~16-bit operand mantissa)'
+DTYPE = 'f32 (storage, LayerNorm, softmax, accumulation); GEMM operands as 2-piece bf16 splits on wgmma (3 products, ~16-bit operand mantissa)'
 
 
 def parse_args():
@@ -56,6 +57,8 @@ def parse_args():
     ap.add_argument('--cpu-steps', type=int, default=3)
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-e2e', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write what the last timed step computed (its four trajectory rows) as '
+                    'DIR/<name>.npy in float32 / float64, so that two builds can be compared output for output')
     a = ap.parse_args()
     for k, v in WORKLOADS[a.workload].items():
         if getattr(a, k) is None:
@@ -106,7 +109,7 @@ def measured_peaks():
             return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
         except Exception:
             pass
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'data sheet (H100 SXM HBM3 3.35 TB/s)'
 
 
 class ClockSampler(threading.Thread):
@@ -226,6 +229,17 @@ def run_reference_arm(a, rank, world):
 
 
 # ------------------------------------------------------------------------------------------------- GPU arm
+def dump_outputs(out_dir, traj, step):
+    """The rows the timed chain wrote for its last step: ligand positions, sampled types, and the v0 / vt log-probabilities
+    (models/molopt_score_model.py:687-693).  Types are integers, stored exactly as float64."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    pos, v, v0, vt = (t[step].cpu() for t in traj)
+    for name, arr in (('pos', pos.numpy().astype(np.float32)), ('v', v.numpy().astype(np.float64)),
+                      ('log_v0', v0.numpy().astype(np.float32)), ('log_vt', vt.numpy().astype(np.float32))):
+        np.save(os.path.join(out_dir, name + '.npy'), arr)
+
+
 def main():
     a = parse_args()
     rank = int(os.environ.get('RANK', 0))
@@ -319,6 +333,8 @@ def main():
     ms = ev0.elapsed_time(ev1)
     launches = lib.tdiff_launch_count(eng) - l0
     clocks = sampler.stop()
+    if rank == 0 and a.dump_outputs:
+        dump_outputs(a.dump_outputs, traj, a.steps - 1)
     if world > 1:
         t = torch.tensor([ms], device=dev, dtype=torch.float64)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -350,13 +366,7 @@ def main():
             else:       # SURVEY.md 8(d): k 512 + v 512 + e_w 4 per edge; q, h, out per node
                 bytes_h, kname = E * 1028 + N * 1536, 'aggregate_h_kernel (fused scatter_softmax->scatter_sum, x2h)'
             ach = bytes_h / t_h / 1e9
-            traffic = None
-            try:        # dram__bytes_read+write of one launch from the committed ncu --set full capture (profiles/, same workload)
-                tj = json.load(open(os.path.join(ROOT, 'profiles', 'aggregate_traffic.json')))
-                if tj.get('kernel', '').startswith(kname.split()[0]) and tj.get('graphs') == G:
-                    traffic = tj['dram_bytes_per_launch']
-            except Exception:
-                pass
+            traffic = None          # DRAM bytes of a launch need a hardware-counter profiler; not measured here
             roofline = {'kernel': kname, 'bound': 'hbm', 'achieved': ach,
                         'peak': peak, 'unit': 'GB/s', 'frac': ach / peak, 'traffic': traffic, 'peak_source': peak_src,
                         'algorithmic_bytes_per_launch': bytes_h, 'avg_launch_ms': t_h * 1e3, 'launches_timed': n_h,
@@ -370,7 +380,7 @@ def main():
                                              'avg_launch_ms': t_x * 1e3, 'share_of_step': ms_x / tot if tot else None}
         if n_mlp:
             # tensor-core work actually executed by the edge MLPs of one layer (x2h: hk + hv on all E rows; h2x: xk + xv on ligand
-            # destinations): per row 3 bf16 products x (128 x NOUT second Linear + 32 x 128 gaussian block) MAC on tcgen05
+            # destinations): per row 3 bf16 products x (128 x NOUT second Linear + 32 x 128 gaussian block) MAC on wgmma
             El = Nl * a.knn
             # (v4: the gaussian/type block of both edge types of a destination class is one K = 64 MMA: 2 x 21 useful slots of 64)
             kpre = 64 if fused else 0
@@ -383,22 +393,14 @@ def main():
                 tpeak = float(json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['bf16_tflops_sustained'])
                 tsrc = 'measured (MEASURED_PEAKS.json bf16_tflops_sustained: kernel timed inside a long step)'
             except Exception:
-                tpeak, tsrc = 1400.0, 'fallback (B200_PROFILING.md sustained 1.4 PFLOP/s)'
+                tpeak, tsrc = 989.0, 'data sheet (H100 SXM dense BF16 989 TFLOP/s)'
             ach = flops / t_m / 1e12
-            # DRAM bytes of one value-MLP (+ aggregation) launch: not measurable inside this run (needs ncu); taken from this round's
-            # committed `ncu --set full` capture of the same workload when there is one, else null
-            mlp_traffic, traffic_src = None, None
-            try:
-                tj = json.load(open(os.path.join(ROOT, 'profiles', 'r02_edge_mlp_traffic.json')))
-                if tj.get('graphs') == G and tj.get('workload') == a.workload:
-                    mlp_traffic, traffic_src = tj['dram_bytes_per_launch'], 'profiles/r02_edge_mlp_traffic.json (ncu --set full, value launch)'
-            except Exception:
-                pass
+            mlp_traffic, traffic_src = None, None     # DRAM bytes need a hardware-counter profiler; not measured here
             extra['edge_mlp'] = {'kernel': 'edge_mlp_v4_kernel x4 per layer (engine mode %d)' % mode, 'bound': 'tensor', 'achieved': ach, 'peak': tpeak,
                                  'unit': 'TFLOP/s', 'frac': ach / tpeak, 'traffic': mlp_traffic, 'traffic_source': traffic_src, 'peak_source': tsrc,
                                  'executed_flops_per_layer': flops, 'useful_flops_per_layer': useful, 'frac_useful': useful / t_m / 1e12 / tpeak,
                                  'ms_per_layer': t_m * 1e3, 'share_of_step': ms_mlp / tot if tot else None,
-                                 'note': 'executed flops = every issued tcgen05 MMA (3 bf16 products per fp32-class product, K = 64 gaussian block '
+                                 'note': 'executed flops = every issued wgmma (3 bf16 products per fp32-class product, K = 64 gaussian block '
                                          'incl. its zero padding); useful = the same without padding slots; the kernel is bound by its '
                                          'CUDA-core LayerNorm/split stage, see DESIGN.md section 6'}
             if roofline is None:            # aggregation fused into the value-MLP epilogue: the dominant kernel is the edge MLP itself
@@ -430,13 +432,7 @@ def main():
             torch.cuda.synchronize(dev)
             t_u = e0.elapsed_time(e1) / reps * 1e-3
             bytes_u = E * 1028 + N * 1536
-            traffic_u = None             # DRAM bytes of one launch from this round's committed ncu capture of the same problem size
-            try:
-                tj = json.load(open(os.path.join(ROOT, 'profiles', 'r02_aggregate_h_traffic.json')))
-                if tj.get('nodes') == N and tj.get('k') == kk:
-                    traffic_u = tj['dram_bytes_per_launch']
-            except Exception:
-                pass
+            traffic_u = None             # DRAM bytes need a hardware-counter profiler; not measured here
             extra['roofline_unfused_aggregate'] = {'kernel': 'aggregate_h_kernel (tdiff_attn_aggregate_h: keys + values from HBM)', 'bound': 'hbm',
                                                    'achieved': bytes_u / t_u / 1e9, 'peak': peak, 'unit': 'GB/s', 'frac': bytes_u / t_u / 1e9 / peak,
                                                    'traffic': traffic_u,
@@ -493,7 +489,7 @@ def main():
                                     'one denoising step of the whole in-flight batch; value = graphs / (1000 * s_per_step)') +
                                    '; all four trajectories written inside the timed region',
                            'parallelism': 'pocket-sharded x%d (no data-path collective)' % world,
-                           'l2': 'per-step working set (k,v edge tensors %.1f GB) >> 126 MB L2; no explicit flush' % (2 * E * 512 / 1e9),
+                           'l2': 'per-step working set (k,v edge tensors %.1f GB) >> 50 MB L2; no explicit flush' % (2 * E * 512 / 1e9),
                            'noise': 'device Philox4x32-10'},
                 'clocks': clocks, 'gpu_launches': int(launches), 'e2e': e2e, 'roofline': roofline, 'cpu_baseline': cpu}
         line.update(extra)

@@ -1,4 +1,4 @@
-/* tdiff.h -- C-ABI of libtdiff.so: the B200 (sm_100a) engine for targetdiff's denoising-sampling hot path.
+/* tdiff.h -- C-ABI of libtdiff.so: the H100 (sm_90a) engine for targetdiff's denoising-sampling hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8(b)).  The reference is pure Python; the "FFI" a maintainer
  * binds is ctypes (see INTEGRATION.md).  Each entry point names the reference interface it replaces
@@ -175,8 +175,8 @@ TDIFF_API int tdiff_check_stability(const float* d_pos, const int32_t* d_atomic_
 /* ---- instrumentation ------------------------------------------------------------------------------------
  * Number of kernel launches issued by this engine since creation (graph replays count their nodes). */
 TDIFF_API int64_t tdiff_launch_count(tdiff_engine* e);
-/* Edge-MLP execution mode of this engine (env TDIFF_EDGE_MLP at creation): 0 FP32 FFMA ("simt"), 2 tcgen05 bf16x2 split with keys in HBM
- * ("tc3v2"), 3 tcgen05 bf16x3 split ("tc6"), 5 tcgen05 bf16x2 split, gaussian block on the tensor core and attention logits fused into the
+/* Edge-MLP execution mode of this engine (env TDIFF_EDGE_MLP at creation): 0 FP32 FFMA ("simt"), 2 wgmma bf16x2 split with keys in HBM
+ * ("tc3v2"), 3 wgmma bf16x3 split ("tc6"), 5 wgmma bf16x2 split, gaussian block on the tensor core and attention logits fused into the
  * key-MLP epilogue (default, "tc3"). */
 TDIFF_API int tdiff_edge_mlp_mode(tdiff_engine* e);
 /* Time (ms, CUDA events on `stream`) and count of the attention-aggregate launches accumulated while profiling is on. */

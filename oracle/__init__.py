@@ -8,7 +8,7 @@ Contents
 --------
 shims/      pure-torch stand-ins for the un-vendored third-party wheels the reference imports
             (torch_scatter 2.1.0, torch_geometric 2.2.0 `knn_graph`, easydict) so that the
-            UNMODIFIED reference `models/*.py` can be imported from /root/reference in the build
+            UNMODIFIED reference `models/*.py` can be imported from a reference checkout in the build
             container (never on the GPU box -- the reference tree does not travel).
 restate.py  op-by-op CPU restatement of the path (every function cites the reference file:line).
 synth.py    seeded synthetic pockets / weights / noise tapes shared by tests and bench.
@@ -21,6 +21,6 @@ The reference ships no tests, golden vectors or checkpoints (SURVEY.md section 4
 is pinned against the reference *itself*, executed here under the shims (tests/test_oracle_vs_reference.py,
 bit-exact) and against committed golden vectors produced by that run (tests/golden/).
 The arithmetic of the third-party kernels (torch_cluster knn tie-breaking / rounding, torch_scatter
-reduction order) is NOT under /root/reference and nothing in the reference pins it:
+reduction order) is NOT in the reference tree and nothing in the reference pins it:
 **parity unpinned at that boundary** -- we fix canonical semantics (SURVEY.md Appendix A.3/A.4).
 """

@@ -1,13 +1,13 @@
-"""Import the UNMODIFIED reference model from /root/reference under the oracle shims.
+"""Import the UNMODIFIED reference model from a reference checkout ($TARGETDIFF_REFERENCE) under the oracle shims.
 
-Test infrastructure; works only where /root/reference exists (the build container).  Nothing run on
-the GPU box (`-m gpu` tests, smoke(), bench.py) may call this.
+Infrastructure for regenerating golden data (oracle/make_golden.py, oracle/make_reference_pins.py); nothing in the
+test-suite, smoke() or bench.py calls it.
 """
 import contextlib
 import os
 import sys
 
-REFERENCE_ROOT = os.environ.get('TARGETDIFF_REFERENCE', '/root/reference')
+REFERENCE_ROOT = os.environ.get('TARGETDIFF_REFERENCE', '')
 SHIMS = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'shims')
 
 

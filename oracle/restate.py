@@ -1,7 +1,7 @@
 """CPU restatement of targetdiff's denoising-sampling hot path (TEST INFRASTRUCTURE, see oracle/__init__.py).
 
 Plain torch-CPU fp32, op by op, working directly on a reference-layout `state_dict` (SURVEY.md
-Appendix D).  Every function cites the reference lines it restates (paths relative to /root/reference).
+Appendix D).  Every function cites the reference lines it restates (paths relative to the reference checkout).
 Randomness never comes from an RNG here: the sampler consumes a *noise tape* (oracle.synth.make_tape)
 in the reference's draw order.
 

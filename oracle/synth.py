@@ -3,7 +3,7 @@
 Synthetic pocket recipe: SURVEY.md section 8(d).  Weights: a deterministic state_dict with the
 reference's 384-entry layout (SURVEY.md Appendix D; reference models/molopt_score_model.py:236-311,
 models/uni_transformer.py:241-274, models/common.py:63-77) drawn from a CPU torch.Generator, so the
-same weights can be rebuilt on the GPU box where /root/reference does not exist.
+same weights can be rebuilt anywhere, without the reference checkout.
 """
 import math
 

@@ -71,7 +71,7 @@ def load():
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise RuntimeError('%s not found: build it with `python -m targetdiff_b200.build` (nvcc, sm_100a). '
+        raise RuntimeError('%s not found: build it with `python -m targetdiff_b200.build` (nvcc, sm_90a). '
                            'targetdiff_b200 has no CPU / PyTorch fallback.' % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

@@ -1,8 +1,8 @@
-"""Build libtdiff.so in-tree with nvcc for sm_100a (no torch involvement: the library only links cudart).
+"""Build libtdiff.so in-tree with nvcc for sm_90a (H100) (no torch involvement: the library only links cudart).
 
     python -m targetdiff_b200.build [--force] [--verbose]
 
-Outputs `targetdiff_b200/libtdiff.so` (git-ignored, but it travels to the GPU box with the gpurun snapshot).
+Outputs `targetdiff_b200/libtdiff.so` (a build product: git-ignored).
 """
 import concurrent.futures
 import os
@@ -18,10 +18,10 @@ _VARIANT = os.environ.get('TDIFF_VARIANT', '')
 OBJ = os.path.join(CSRC, 'build' + ('_' + _VARIANT if _VARIANT else ''))
 LIB = os.path.join(HERE, 'libtdiff%s.so' % ('_' + _VARIANT if _VARIANT else ''))
 SOURCES = ['engine.cu', 'knn.cu', 'edge_const.cu', 'node_ops.cu', 'edge_mlp.cu', 'edge_mlp_tc.cu', 'edge_mlp_v4.cu', 'aggregate.cu', 'sampler.cu', 'stability.cu']
-HEADERS = ['tdiff_common.cuh', 'sampler.cuh', os.path.join('..', '..', 'include', 'tdiff.h')]
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
+HEADERS = ['tdiff_common.cuh', 'sampler.cuh', 'hopper_mma.cuh', os.path.join('..', '..', 'include', 'tdiff.h')]
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
               '-Xcompiler', '-fvisibility=hidden', '-Xptxas', '-v']
-# developer switch, e.g. TDIFF_NVCC_EXTRA=-DTDIFF_V3_TIMELINE (clock64 timeline stamps in edge_mlp_v3, see tools/v3_timeline.py)
+# developer switch: extra nvcc flags, e.g. TDIFF_NVCC_EXTRA=-DNDEBUG
 NVCC_FLAGS += os.environ.get('TDIFF_NVCC_EXTRA', '').split()
 
 
@@ -66,7 +66,7 @@ def build(force=False, verbose=False):
                 f.write(r.stdout + r.stderr)
     objs = [os.path.join(OBJ, s.replace('.cu', '.o')) for s in SOURCES]
     if force or jobs or _stale(LIB, objs):
-        cmd = [nvcc, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB] + objs
+        cmd = [nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB] + objs
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)

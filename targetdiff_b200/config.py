@@ -46,7 +46,7 @@ def default_sampling_config():
                                 sample_num_atoms='prior'))
 
 
-# Values the sm_100a engine implements; anything else is rejected loudly (SURVEY.md 8(b) "should-reject-clearly").
+# Values the sm_90a engine implements; anything else is rejected loudly (SURVEY.md 8(b) "should-reject-clearly").
 _SUPPORTED = dict(model_mean_type=('C0', 'noise'), beta_schedule=('sigmoid', 'linear', 'quad', 'const', 'jsd', 'cosine'),
                   v_beta_schedule=('cosine',), node_indicator=(True,), model_type=('uni_o2',),
                   hidden_dim=(128,), n_heads=(16,), edge_feat_dim=(4,), num_r_gaussian=(20,), act_fn=('relu',),
@@ -61,7 +61,7 @@ _WHY_NOT = {
 def check_supported(cfg):
     for k, allowed in _SUPPORTED.items():
         if k in cfg and cfg[k] not in allowed:
-            raise NotImplementedError('config %s=%r is not implemented by the B200 engine (supported: %s)%s' % (
+            raise NotImplementedError('config %s=%r is not implemented by the H100 engine (supported: %s)%s' % (
                 k, cfg[k], list(allowed), '; ' + _WHY_NOT[k] if k in _WHY_NOT else ''))
     if not (1 <= int(cfg.knn) <= 64):
         raise NotImplementedError('knn=%r outside 1..64' % (cfg.knn,))

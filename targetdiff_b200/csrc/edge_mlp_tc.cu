@@ -1,31 +1,29 @@
-// edge_mlp_tc.cu -- per-edge MLPs with the second Linear on the 5th-gen tensor cores (tcgen05 + TMEM), fp32-faithful.
+// edge_mlp_tc.cu -- per-edge MLPs and node-side GEMMs with the second Linear on the Hopper tensor cores (wgmma), fp32-faithful.
 //
 // Same math as edge_mlp.cu (reference models/uni_transformer.py:45-56,111-120 + models/common.py:60-80 after the exact
 // first-layer split of SURVEY.md Appendix B); different execution:
 //
 //   * the [128 edges x 128] hidden tile and the [128 x 128] weight are split into NP bf16 pieces each
-//     (x = x1 + x2 (+ x3), xi = bf16(residual)); the product is recovered with 3 (NP=2) or 6 (NP=3) tcgen05.mma
-//     kind::f16 passes accumulating in fp32 in TMEM:  a1b1 + a1b2 + a2b1 (+ a1b3 + a2b2 + a3b1).
+//     (x = x1 + x2 (+ x3), xi = bf16(residual)); the product is recovered with 3 (NP=2) or 6 (NP=3) wgmma
+//     bf16 passes accumulating in fp32 registers:  a1b1 + a1b2 + a2b1 (+ a1b3 + a2b2 + a3b1).
 //     NP=3 keeps 24 mantissa bits of both operands (error ~2^-22, i.e. fp32 GEMM class); NP=2 keeps 16.
 //     Plain TF32 / BF16 single-pass MMA would break the 1e-4 position tolerance (SURVEY.md section 7).
-//   * warp-specialised persistent CTA (one per SM), roles aligned to warpgroups so setmaxnreg can hand registers to producers:
-//       warps 0-3   epilogue: tcgen05.ld accumulator rows (warp q owns TMEM lanes 32q..32q+31) -> +bias -> global
-//       warp  4     TMEM allocator + single-thread MMA issuer (tcgen05.mma / tcgen05.commit); warps 5-7 idle
-//       warps 8..   producers, 8 warps per set (NSETS sets work on different tiles concurrently):
-//                   8 edge rows per warp in registers -- coalesced 512 B gathers of the projected node
+//   * warp-specialised persistent CTA (one per SM):
+//       warps 0-7   two consumer warpgroups: warpgroup g issues the wgmma of tile rows 64g..64g+63 and stores its accumulator
+//                   fragment (+bias) straight to global memory
+//       warps 8-15  producers: 8 edge rows per warp in registers -- coalesced 512 B gathers of the projected node
 //                   rows, gaussians by 4 lanes per row, type/gaussian table through L1 (one table row feeds 8 edge rows),
-//                   LayerNorm by shuffles, ReLU, bf16 split, 8-byte stores into the UMMA K-major SWIZZLE_128B layout
-//     mbarriers: a_full/a_empty (producers <-> MMA), d_full/d_empty (MMA <-> epilogue, accumulator double-buffered in TMEM).
+//                   LayerNorm by shuffles, ReLU, bf16 split, 8-byte stores into the K-major SWIZZLE_128B layout
+//     mbarriers: a_full/a_empty (producers <-> consumers), activation tiles multi-buffered (NBUF).
 //   * the weight pieces are pre-swizzled on the host into the exact shared-memory image (engine.cu: pack_umma_image).
 //
 // Shared memory: NP*32 KB weights + NBUF*NP*32 KB activation tiles (+2 KB) -> 194 KB for (NP=3,NBUF=1) and (NP=2,NBUF=2).
 #include "tdiff_common.cuh"
+#include "hopper_mma.cuh"
 
 namespace {
 
-// warp roles (warpgroup-aligned so that setmaxnreg can move registers from the light roles to the producers)
-constexpr int kEpiWarps = 4;       // warps 0-3
-constexpr int kMmaWarp = 4;        // warp 4 (warps 5-7 idle: they only keep the warpgroup aligned)
+constexpr int kConsWarps = 8;      // warps 0-7: two consumer warpgroups (64 rows each)
 constexpr int kProdWarp0 = 8;      // warps 8.. : producers, 8 warps per producer set
 constexpr int kProdWarps = 8;      // warps per producer set == arrivals per activation tile
 constexpr int kPieceBytes = 128 * 128 * 2;                 // one bf16 piece of a 128x128 tile
@@ -53,50 +51,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] . B[smem]^T ; bf16 inputs, fp32 accumulate, M=128, N=128, K=16 per instruction
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// UMMA shared-memory descriptor, K-major, SWIZZLE_128B, 8-row groups 1024 B apart (cute::UMMA::SmemDescriptor fields:
-// start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout_type=2 (SWIZZLE_128B) [61,64))
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1<<4), a/b format BF16 (1<<7, 1<<10), K-major both,
-// N>>3 at [17,23), M>>4 at [24,29)
-constexpr uint32_t kIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
 
 // two fp32 -> packed bf16x2 (round-to-nearest-even): `lo` in bits [0,16), `hi` in bits [16,32)
 __device__ __forceinline__ uint32_t cvt_bf16x2(float hi, float lo) {
@@ -121,12 +75,10 @@ __device__ __forceinline__ float4 ldg_stream(const float* p) {
   return v;
 }
 
-// packed fp32 FMA (Blackwell FFMA2): (d0, d1) += w * (a0, a1)
+// (d0, d1) += w * (a0, a1), two fused multiply-adds
 __device__ __forceinline__ void ffma2(float& d0, float& d1, float w, float a0, float a1) {
-  asm("{\n\t.reg .b64 ww, aa, dd;\n\tmov.b64 ww, {%2, %2};\n\tmov.b64 aa, {%3, %4};\n\tmov.b64 dd, {%0, %1};\n\t"
-      "fma.rn.f32x2 dd, ww, aa, dd;\n\tmov.b64 {%0, %1}, dd;\n\t}"
-      : "+f"(d0), "+f"(d1)
-      : "f"(w), "f"(a0), "f"(a1));
+  d0 = __fmaf_rn(w, a0, d0);
+  d1 = __fmaf_rn(w, a1, d1);
 }
 
 template <int NP>
@@ -145,20 +97,6 @@ __device__ __forceinline__ void split_store_row(uint32_t a_tile, int row, int la
 }
 
 }  // namespace
-
-template <int REGS> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
-template <int REGS> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
-
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {   // for roles that are not on the critical path
-  uint32_t done = 0;
-  while (true) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (done) break;
-    __nanosleep(200);
-  }
-}
 
 // MODE 0: edge MLP (gathers + gaussian block + LN + ReLU -> second Linear), out [n_rows,128]
 // MODE 1: dense rows: out[:, y*128:(y+1)*128] = in[:, :128] . W_y^T + b_y for column block y = blockIdx.y (node projection)
@@ -184,20 +122,14 @@ edge_mlp_tc_kernel(const float* __restrict__ P, const float4* __restrict__ xm, c
   float* s_b2 = reinterpret_cast<float*>(sA + NBUF * NP * kPieceBytes);   // [128]
   float* s_g = s_b2 + TD_H;
   float* s_b = s_g + TD_H;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_b + TD_H);  // a_full[NBUF], a_empty[NBUF], d_full[2], d_empty[2]
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + 2 * NBUF + 4);
-  const uint32_t bar_a_full = smem_u32(bars), bar_a_empty = smem_u32(bars + NBUF), bar_d_full = smem_u32(bars + 2 * NBUF),
-                 bar_d_empty = smem_u32(bars + 2 * NBUF + 2);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_b + TD_H);  // a_full[NBUF], a_empty[NBUF]
+  const uint32_t bar_a_full = smem_u32(bars), bar_a_empty = smem_u32(bars + NBUF);
 
   // the warp index is broadcast from lane 0 so that the compiler KNOWS it is warp-uniform: role branches become uniform branches and
   // every constant-bank read indexed by it (LayerNorm parameters, biases) goes through the uniform datapath (LDCU + UR operands)
   // instead of per-thread LDC into vector registers
-#ifdef TDIFF_PLAIN_WARP_INDEX          // A/B switch (tools/build_variant.sh): the pre-change form, per-thread LDC
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-#else
   const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-#endif
-  // ---- one-time setup: weights image -> smem, params, barriers, TMEM
+  // ---- one-time setup: weights image -> smem, params, barriers
   constexpr int kThreads = (kProdWarp0 + kProdWarps * NSETS) * 32;
   static_assert(NBUF >= NSETS, "every producer set needs its own activation buffer");
   for (int i = tid; i < NP * kPieceBytes / 16; i += kThreads)
@@ -209,20 +141,12 @@ edge_mlp_tc_kernel(const float* __restrict__ P, const float4* __restrict__ xm, c
   if (tid == 0) {
     for (int i = 0; i < NBUF; ++i) {
       mbar_init(bar_a_full + 8 * i, kProdWarps);
-      mbar_init(bar_a_empty + 8 * i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar_d_full + 8 * i, 1);
-      mbar_init(bar_d_empty + 8 * i, kEpiWarps);
+      mbar_init(bar_a_empty + 8 * i, kConsWarps);
     }
     fence_barrier_init();
   }
-  if (warp == kMmaWarp) tmem_alloc(smem_u32(s_tmem), 256);
   fence_proxy_async();            // weight image (generic-proxy stores) -> visible to the tensor-core (async) proxy
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
   if (MODE != 0 && rw.d_n_rows) n_rows = *rw.d_n_rows;
   const long long n_tiles = (n_rows + 127) / 128;
@@ -232,7 +156,6 @@ edge_mlp_tc_kernel(const float* __restrict__ P, const float4* __restrict__ xm, c
     // =============================================================== producers
     // Producer set `ps` (8 warps) builds the activation tiles of the CTA's local tiles it = ps, ps+NSETS, ...; inside a set,
     // warp pw owns rows pw*16 .. pw*16+15 as two "groups" of 8 rows held in registers.
-    if (NSETS > 1) reg_inc<96>();
     const int ps = (warp - kProdWarp0) / kProdWarps, pw = (warp - kProdWarp0) % kProdWarps;
     if constexpr (MODE != 0) {
       // ---- dense / LN row producers: 8 rows per warp-iteration straight from `in` (coalesced 512 B rows)
@@ -405,79 +328,49 @@ edge_mlp_tc_kernel(const float* __restrict__ P, const float4* __restrict__ xm, c
       s0 = s1; t0 = t1; d0 = d1; dist0 = dist1;
     }
     }
-  } else if (warp >= kMmaWarp) {
-    // =============================================================== MMA issuer (one thread of warp 4; warps 5-7 idle)
-    if (NSETS > 1) reg_dec<32>();        // executed by the whole warpgroup (warps 4-7)
-    for (long long it = 0; warp == kMmaWarp && it < my_tiles; ++it) {
-      const int buf = (int)(it % NBUF);
-      const uint32_t pha = (uint32_t)((it / NBUF) & 1);
-      const int db = (int)(it & 1);
-      const uint32_t phd = (uint32_t)((it >> 1) & 1);
-      mbar_wait_relaxed(bar_d_empty + 8 * db, phd ^ 1);  // accumulator buffer drained by the epilogue
-      mbar_wait_relaxed(bar_a_full + 8 * buf, pha);      // activation tile written
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t a_addr = smem_u32(sA + buf * NP * kPieceBytes), b_addr = smem_u32(sB);
-        const uint32_t d_addr = tmem_base + (uint32_t)db * 128;
-        uint32_t accum = 0;
-        // terms (pa, pb) with pa + pb <= NP-1:  a1b1 | a1b2, a2b1 | a1b3, a2b2, a3b1 ; smallest contributions last
-#pragma unroll
-        for (int sum = 0; sum < NP; ++sum) {
-#pragma unroll
-          for (int pa = 0; pa <= sum; ++pa) {
-            const int pb = sum - pa;
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk) {             // K = 128 in 8 instructions of K=16 (32 B inside a 128 B swizzle row)
-              const uint32_t koff = (kk >> 2) * kAtomBytes + (kk & 3) * 32;
-              umma_bf16(d_addr, umma_desc_k_sw128(a_addr + pa * kPieceBytes + koff), umma_desc_k_sw128(b_addr + pb * kPieceBytes + koff),
-                        kIdesc, accum);
-              accum = 1;
-            }
-          }
-        }
-        umma_commit(bar_a_empty + 8 * buf);              // activation tile may be overwritten once these MMAs retire
-        umma_commit(bar_d_full + 8 * db);                // accumulator ready for the epilogue
-      }
-      __syncwarp();
-    }
   } else {
-    // =============================================================== epilogue (warps 0..3 <-> TMEM lanes 32w..32w+31)
-    if (NSETS > 1) reg_dec<64>();   // budget: 128*64 + 128*32 + 512*96 = 61440 = the 768 x 80 registers the CTA was launched with
+    // =============================================================== consumers: warpgroup g = rows 64g..64g+63 of every tile
+    const int g = warp >> 2, wq = warp & 3;
     for (long long it = 0; it < my_tiles; ++it) {
       const long long tile = blockIdx.x + it * gridDim.x;
-      const int db = (int)(it & 1);
-      const uint32_t phd = (uint32_t)((it >> 1) & 1);
-      mbar_wait_relaxed(bar_d_full + 8 * db, phd);
-      tc_fence_after();
-      const long long idx = tile * 128 + warp * 32 + lane;
-      const long long orow_i = (MODE != 0 && rw.row_list && idx < n_rows) ? rw.row_list[idx] : idx;
-      float* orow = out + (size_t)orow_i * (MODE == 0 ? 128 : rw.ldo) + (MODE == 1 ? blockIdx.y * 128 : 0);
-#pragma unroll 1
-      for (int c0 = 0; c0 < 128; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(db * 128 + c0), v);
-        if (idx < n_rows) {
+      const int buf = (int)(it % NBUF);
+      mbar_wait(bar_a_full + 8 * buf, (uint32_t)((it / NBUF) & 1));      // activation tile written
+      const uint32_t a_addr = smem_u32(sA + buf * NP * kPieceBytes) + (uint32_t)g * 64u * 128u, b_addr = smem_u32(sB);
+      float d[64];
+      wgmma_fence();
+      uint32_t accum = 0;
+      // terms (pa, pb) with pa + pb <= NP-1:  a1b1 | a1b2, a2b1 | a1b3, a2b2, a3b1 ; smallest contributions last
 #pragma unroll
-          for (int c = 0; c < 32; c += 8) {          // 32-byte stores: one full sector per thread
-            const float4 ba = lds128(smem_u32(s_b2 + c0 + c)), bb = lds128(smem_u32(s_b2 + c0 + c + 4));
-            asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(orow + c0 + c), "f"(__uint_as_float(v[c]) + ba.x),
-                         "f"(__uint_as_float(v[c + 1]) + ba.y), "f"(__uint_as_float(v[c + 2]) + ba.z), "f"(__uint_as_float(v[c + 3]) + ba.w),
-                         "f"(__uint_as_float(v[c + 4]) + bb.x), "f"(__uint_as_float(v[c + 5]) + bb.y), "f"(__uint_as_float(v[c + 6]) + bb.z),
-                         "f"(__uint_as_float(v[c + 7]) + bb.w) : "memory");
+      for (int sum = 0; sum < NP; ++sum) {
+#pragma unroll
+        for (int pa = 0; pa <= sum; ++pa) {
+          const int pb = sum - pa;
+#pragma unroll
+          for (int kk = 0; kk < 8; ++kk) {             // K = 128 in 8 instructions of K=16 (32 B inside a 128 B swizzle row)
+            const uint32_t koff = (kk >> 2) * kAtomBytes + (kk & 3) * 32;
+            wgmma_n128(d, gmma_desc_sw128(a_addr + pa * kPieceBytes + koff), gmma_desc_sw128(b_addr + pb * kPieceBytes + koff), accum);
+            accum = 1;
           }
         }
       }
-      tc_fence_before();
+      wgmma_commit();
+      wgmma_wait_all();
       __syncwarp();
-      if (lane == 0) mbar_arrive(bar_d_empty + 8 * db);
+      if (lane == 0) mbar_arrive(bar_a_empty + 8 * buf);        // activation tile may be overwritten
+      // ---- fragment -> global: rows r0 and r0 + 8, columns 8i + 2 (lane % 4) + {0, 1}
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long long idx = tile * 128 + 64 * g + 16 * wq + (lane >> 2) + 8 * h;
+        if (idx >= n_rows) continue;
+        const long long orow_i = (MODE != 0 && rw.row_list) ? rw.row_list[idx] : idx;
+        float* orow = out + (size_t)orow_i * (MODE == 0 ? 128 : rw.ldo) + (MODE == 1 ? blockIdx.y * 128 : 0);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          const int c = 8 * i + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(orow + c) = make_float2(d[4 * i + 2 * h] + s_b2[c], d[4 * i + 2 * h + 1] + s_b2[c + 1]);
+        }
+      }
     }
-  }
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 
@@ -485,7 +378,7 @@ template <int NP, int NBUF, int NSETS, int MODE>
 static void launch_tc(const float* P, const float4* xm, const int* src, const unsigned char* etype, const float* dist, const int* row_nodes,
                       long long n_rows, int k, TdMlp m, const unsigned char* w2_image, const float* offsets, float coeff, float* out, TcRows rw,
                       int nblocks, int sm_count, cudaStream_t st) {
-  const size_t smem = 1024 + (size_t)NP * kPieceBytes + (size_t)NBUF * NP * kPieceBytes + 3 * TD_H * sizeof(float) + (2 * NBUF + 4) * 8 + 16;
+  const size_t smem = 1024 + (size_t)NP * kPieceBytes + (size_t)NBUF * NP * kPieceBytes + 3 * TD_H * sizeof(float) + 2 * NBUF * 8;
   static size_t opted[TD_MAX_DEVICES] = {0};
   td_opt_in_smem(edge_mlp_tc_kernel<NP, NBUF, NSETS, MODE>, smem, opted);
   const long long n_tiles = (n_rows + 127) / 128;
@@ -502,7 +395,7 @@ void td_launch_edge_mlp_tc(const float* P, const float4* xm, const int* src, con
                            float* out, int sm_count, cudaStream_t st) {
   if (n_rows == 0) return;
   TcRows rw = {nullptr, 0, 0, 128, nullptr, nullptr};
-  if (pieces == 2) launch_tc<2, 2, 2, 0>(P, xm, src, etype, dist, row_nodes, n_rows, k, m, w2_image, offsets, coeff, out, rw, 1, sm_count, st);
+  if (pieces == 2) launch_tc<2, 2, 1, 0>(P, xm, src, etype, dist, row_nodes, n_rows, k, m, w2_image, offsets, coeff, out, rw, 1, sm_count, st);
   else launch_tc<3, 1, 1, 0>(P, xm, src, etype, dist, row_nodes, n_rows, k, m, w2_image, offsets, coeff, out, rw, 1, sm_count, st);
 }
 
@@ -514,10 +407,10 @@ void td_launch_rows_tc(int mode, const float* in, int ldi, int in_off, long long
   if (n_rows == 0) return;          // with d_n_rows, n_rows is only the upper bound used to size the grid
   TcRows rw = {in, ldi, in_off, ldo, row_list, d_n_rows};
   if (mode == 1) {
-    if (pieces == 2) launch_tc<2, 2, 2, 1>(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, n_rows, 1, m, w_image, nullptr, 0.f, out, rw, nblocks, sm_count, st);
+    if (pieces == 2) launch_tc<2, 2, 1, 1>(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, n_rows, 1, m, w_image, nullptr, 0.f, out, rw, nblocks, sm_count, st);
     else launch_tc<3, 1, 1, 1>(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, n_rows, 1, m, w_image, nullptr, 0.f, out, rw, nblocks, sm_count, st);
   } else {
-    if (pieces == 2) launch_tc<2, 2, 2, 2>(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, n_rows, 1, m, w_image, nullptr, 0.f, out, rw, 1, sm_count, st);
+    if (pieces == 2) launch_tc<2, 2, 1, 2>(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, n_rows, 1, m, w_image, nullptr, 0.f, out, rw, 1, sm_count, st);
     else launch_tc<3, 1, 1, 2>(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, n_rows, 1, m, w_image, nullptr, 0.f, out, rw, 1, sm_count, st);
   }
 }

@@ -1,48 +1,44 @@
-// edge_mlp_v4.cu -- per-edge MLP, fourth generation (default): every edge type's gaussian block on tcgen05, activations handed to
-// the second Linear through tensor memory.
+// edge_mlp_v4.cu -- per-edge MLP, fourth generation (default): both Linear layers and every edge type's gaussian block on the Hopper
+// tensor cores (wgmma), fp32-faithful through bf16 operand splitting.
 //
 // Math (reference models/uni_transformer.py:45-56,111-120, models/common.py:60-80 after the exact first-layer split, SURVEY App. B):
 //   pre[e]  = P[dst, offA:+128] + P[src, offB:+128] + tab[type][20] + sum_j g_j(dist_e) * tab[type][j]
 //   hid     = relu(LN(pre) * ln_g + ln_b)
 //   out[e]  = hid . W2^T + b2
 //
-// What changed against edge_mlp_v3.cu (kept for the history in git):
 //   * rows are visited through a CLASS-SORTED destination list (protein destinations, padded to a tile multiple, then ligand
-//     destinations): a 128-row tile holds destinations of one class, hence at most two edge types -- protein destination: P->P (3) or
+//     destinations): a tile holds destinations of one class, hence at most two edge types -- protein destination: P->P (3) or
 //     L->P (1); ligand destination: P->L (2) or L->L (0).  The gaussian/type block of BOTH is one small MMA
-//         Dpre[128 x 128] = G[128 x 64] . TabClass^T,   G row = (g_0..g_19, 1, 0..) in the 32-slot half of the row's own type,
-//     so the CUDA-core pre-pass for the "rare" types (edge_slow_kernel, 13 % of the step) and its 3.4 GB row buffer are gone;
-//   * the activation operand A of the second Linear never touches shared memory: row threads (thread = accumulator row) write their
-//     bf16 pieces with tcgen05.st into tensor memory and the MMA reads A from there (no swizzle arithmetic, no proxy fence);
-//   * LayerNorm statistics are exchanged through two slot sets (2 named barriers per tile instead of 4); the staging tile uses a
-//     padded row stride instead of an XOR swizzle (immediate-offset loads); LayerNorm affine parameters are read as 128-bit
-//     constant loads.
+//         Dpre[64 x 128] = G[64 x 64] . TabClass^T,   G row = (g_0..g_19, 1, 0..) in the 32-slot half of the row's own type;
+//   * both MMAs run on one warpgroup (wgmma, operands in shared memory, fp32 accumulators in registers); it hands Dpre and D to the
+//     CUDA-core roles as row-major fp32 tiles in shared memory, so those roles keep thread = row;
+//   * LayerNorm statistics are exchanged through two slot sets (2 named barriers per tile).
 //
-// CTA = 28 warps, one CTA per SM, persistent over tiles of 128 edge rows:
-//   warps  0-7   epilogue      TMEM D -> +b2 -> logits / softmax weights / fused attention aggregation / plain rows   (72 regs)
-//   warps  8-11  gather        32 rows each: cp.async 512 B rows of P[src] -> S; warp 11 also issues the MMAs          (40)
-//   warps 12-27  row threads   warp 12+q+4*qq: rows 32q..32q+31, feature quarter qq                                   (80)
-// Shared memory (197 KB): W2 pieces 64 KB | S fp32 72 KB (row stride 144 B) | G pieces 32 KB | class table pieces 32 KB | 4 KB exchange.
-// TMEM 512 columns: D[2] at 0/128, Dpre at 256, A pieces at 384 / 448.  bf16 split: 2 pieces / 3 products (a1b1 + a1b2 + a2b1).
+// CTA = 16 warps (512 threads), one CTA per SM, persistent over tiles of 64 edge rows (one wgmma M):
+//   warps  0-3   MMA warpgroup  Dpre and D wgmma, accumulator fragments -> shared memory
+//   warps  4-7   epilogue       D -> +b2 -> logits / softmax weights / fused attention aggregation / plain rows
+//   warps  8-15  row threads    warp 8+q+2*qq: rows 32q..32q+31, feature quarter qq; gathers P[src] / P[dst] straight from L2
+// Shared memory (212 KB): W2 pieces 64 KB | class table pieces 32 KB | G pieces 16 KB | A pieces 32 KB | Dpre 33 KB | D 33 KB | exchange 2 KB.
+// bf16 split: 2 pieces / 3 products (a1b1 + a1b2 + a2b1).
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include "tdiff_common.cuh"
+#include "hopper_mma.cuh"
 
 namespace v4 {
 
-constexpr int kThreads = 28 * 32;
-constexpr int kEpiWarps = 8, kGatherWarp0 = 8, kGatherWarps = 4, kMmaWarp = 11, kRowWarp0 = 12, kRowWarps = 16;
-constexpr int kAtom = 128 * 128;           // 128 rows x 128 B: one SWIZZLE_128B K-block of a 128-row operand
-constexpr int kSRow = 144;                 // staging row stride (128 B of data + 16 B pad: conflict-free thread-per-row reads)
-constexpr int kSAtom = 128 * kSRow;        // one feature quarter of the staging tile
-constexpr int kTabClassBytes = 2 * kAtom;  // one class table: 2 bf16 pieces of [128 x 64]
+constexpr int kThreads = 16 * 32;
+constexpr int kTile = 64;                  // rows per tile
+constexpr int kMmaWarps = 4, kEpiWarp0 = 4, kEpiWarps = 4, kRowWarp0 = 8, kRowWarps = 8;
+constexpr int kGAtom = kTile * 128;        // one SWIZZLE_128B K-block (64 bf16) of a 64-row operand
+constexpr int kTabClassBytes = 2 * 128 * 128;   // one class table: 2 bf16 pieces of [128 x 64]
+constexpr int kDRow = 132;                 // fp32 row stride of the Dpre / D tiles (conflict-free 16-byte thread-per-row reads)
 // shared-memory map (bytes from the 1024-aligned base)
-constexpr int oW = 0, oG = oW + 4 * kAtom, oT = oG + 2 * kAtom, oS = oT + 2 * kAtom, oX = oS + 4 * kSAtom, oBar = oX + 2 * 2048,
-              kSmem = oBar + 16 * 8 + 16;
-enum { B_S_FULL = 0, B_S_EMPTY, B_G_FULL, B_A_FULL, B_A_EMPTY, B_DPRE_FULL, B_D_FULL0, B_D_FULL1, B_D_EMPTY0, B_D_EMPTY1, B_LOAD, B_TAB };
-constexpr uint32_t kColD = 0, kColDpre = 256, kColA = 384;
+constexpr int oW = 0, oT = oW + 4 * 128 * 128, oG = oT + kTabClassBytes, oA = oG + 2 * kGAtom, oDp = oA + 4 * kGAtom,
+              oD = oDp + kTile * kDRow * 4, oX = oD + kTile * kDRow * 4, oBar = oX + 2 * 4 * kTile * 4, kSmem = oBar + 16 * 8;
+enum { B_G_FULL = 0, B_DPRE_FULL, B_A_FULL, B_A_EMPTY, B_D_FULL, B_D_EMPTY, B_LOAD, B_TAB };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -63,7 +59,7 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity)
     __nanosleep(100);
   }
 }
-// TMA bulk copy (1-D): global -> shared, completion counted in bytes on an mbarrier (SASS: UBLKCP + SYNCS.ARRIVE.TRANS64)
+// TMA bulk copy (1-D): global -> shared, completion counted in bytes on an mbarrier
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -73,76 +69,7 @@ __device__ __forceinline__ void bulk_g2s(uint32_t smem_dst, const void* gsrc, ui
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-template <int REGS> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
-template <int REGS> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] . B[smem desc]
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-               "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// D[tmem] (+)= A[tmem] . B[smem desc]   (A: lane = row, 16-bit elements packed two per 32-bit column, K contiguous)
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-               "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// One elected lane of a converged warp.  Unlike `lane == 0`, the compiler knows that a branch on elect.sync is single-threaded: the
-// uniform-datapath instructions under it (tcgen05.mma, tcgen05.commit) are issued back to back instead of inside a per-lane election
-// loop (6 instructions per MMA) -- the MMA-issuing warp is the one the row threads wait for.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  tmem_ld16_nowait(taddr, r);
-  tmem_ld_wait();
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-  tmem_ld_wait();
-}
-// 16 x 32-bit registers of this thread -> its TMEM lane, 16 consecutive columns
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr), "r"(r[0]),
-      "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]),
-      "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-// K-major SWIZZLE_128B UMMA descriptor (8-row groups 1024 B apart)
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t a) {
-  return (uint64_t)((a >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-constexpr uint32_t kIdesc128 = (1u << 4) | (1u << 7) | (1u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);   // bf16 x bf16 -> f32, M=N=128
 
 __device__ __forceinline__ uint32_t cvt_bf16x2(float hi, float lo) {
   uint32_t d;
@@ -152,8 +79,8 @@ __device__ __forceinline__ uint32_t cvt_bf16x2(float hi, float lo) {
 __device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
-__device__ __forceinline__ void sts128f(uint32_t addr, float4 v) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+__device__ __forceinline__ void sts64f(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
   float4 v;
@@ -166,23 +93,43 @@ __device__ __forceinline__ float lds32f(uint32_t addr) {
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
   return v;
 }
-__device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gsrc) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gsrc) : "memory");
+// N consecutive fp32 of a Dpre / D row as raw bits
+template <int N>
+__device__ __forceinline__ void lds_row(uint32_t addr, uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; i += 4) {
+    const float4 v = lds128(addr + 4u * (uint32_t)i);
+    r[i] = __float_as_uint(v.x); r[i + 1] = __float_as_uint(v.y); r[i + 2] = __float_as_uint(v.z); r[i + 3] = __float_as_uint(v.w);
+  }
 }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+__device__ __forceinline__ void lds16(uint32_t addr, uint32_t (&r)[16]) { lds_row<16>(addr, r); }
+__device__ __forceinline__ void lds32(uint32_t addr, uint32_t (&r)[32]) { lds_row<32>(addr, r); }
 __device__ __forceinline__ void stg256(float* p, float a, float b, float c, float d, float e, float f, float g, float h) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d), "f"(e), "f"(f), "f"(g), "f"(h) : "memory");
+  asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+  asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p + 4), "f"(e), "f"(f), "f"(g), "f"(h) : "memory");
 }
-// packed fp32 pairs (Blackwell FADD2 / FFMA2)
-typedef unsigned long long f2;
-__device__ __forceinline__ f2 pk2(float a, float b) { f2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(f2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) { f2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f2 sub2(f2 a, f2 b) { f2 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) { f2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { f2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+// fp32 pairs, each lane of the pair rounded on its own (the order of operations is the kernel's, not the compiler's)
+typedef float2 f2;
+__device__ __forceinline__ f2 pk2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void upk2(f2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 sub2(f2 a, f2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+
+// accumulator fragment of one m64nNk16 warpgroup MMA -> row-major fp32 tile (row stride kDRow)
+template <int N>
+__device__ __forceinline__ void store_frag(uint32_t tile, const float (&d)[N / 2], int wq, int lane) {
+  const uint32_t r0 = (uint32_t)(16 * wq + (lane >> 2));
+#pragma unroll
+  for (int i = 0; i < N / 8; ++i) {
+    const uint32_t c = (uint32_t)(8 * i + 2 * (lane & 3));
+    sts64f(tile + 4u * (r0 * kDRow + c), d[4 * i], d[4 * i + 1]);
+    sts64f(tile + 4u * ((r0 + 8u) * kDRow + c), d[4 * i + 2], d[4 * i + 3]);
+  }
+}
 
 // LayerNorm affine parameters and the output bias travel as a kernel argument (constant bank, read with 128-bit loads)
 struct LnParams { float4 g4[32]; float4 b4[32]; float b2[128]; float mu[20]; };
@@ -225,39 +172,7 @@ __device__ __forceinline__ void split2(float y0, float y1, uint32_t& hi, uint32_
 
 }  // namespace v4
 
-// In-situ wait accounting (variant build only: TDIFF_NVCC_EXTRA=-DTDIFF_WAIT_STATS, tools/wait_stats.py): SM clock cycles the roles
-// spend in their mbarrier waits, summed over every edge_mlp_v4 launch since the last reset.  Slots: 0 row loop total, 1 row S_FULL,
-// 2 row DPRE_FULL, 3 row A_EMPTY, 4 gather loop total, 5 gather S_EMPTY, 6 gather copy (issue + cp.async completion),
-// 7 MMA warp G_FULL, 8 MMA warp D_EMPTY + A_FULL, 9 epilogue loop total, 10 epilogue D_FULL, 11-13 warp loops counted (row, gather,
-// epilogue), 14 MMA warp loop total, 15 MMA warp S_EMPTY
-#ifdef TDIFF_WAIT_STATS
-__device__ unsigned long long g_wait_stats[16];
-#define WS_DECL(n) unsigned ws_##n = 0
-#define WS_T0() const unsigned ws_c0 = (unsigned)clock()
-#define WS_ADD(n) ws_##n += (unsigned)clock() - ws_c0
-#define WS_FLUSH(slot, n) do { if (lane == 0) atomicAdd(&g_wait_stats[slot], (unsigned long long)ws_##n); } while (0)
-extern "C" __attribute__((visibility("default"))) int tdiff_debug_wait_stats(unsigned long long* out16, int reset) {
-  if (out16 && cudaMemcpyFromSymbol(out16, g_wait_stats, sizeof(unsigned long long) * 16) != cudaSuccess) return -1;
-  if (reset) {
-    unsigned long long z[16] = {0};
-    if (cudaMemcpyToSymbol(g_wait_stats, z, sizeof(z)) != cudaSuccess) return -1;
-  }
-  return 0;
-}
-#else
-#define WS_DECL(n)
-#define WS_T0()
-#define WS_ADD(n)
-#define WS_FLUSH(slot, n)
-#endif
-
 using namespace v4;
-
-#ifdef TDIFF_LANE0_MMA           // A/B switch: the pre-change form
-#define MMA_LANE (lane == 0)
-#else
-#define MMA_LANE elect_one()
-#endif
 
 // NOUT = 128: key / value MLPs (hk, hv, xk);  NOUT = 16: the per-head scalar value MLP of h2x (xv).
 // Rows: idx = a * k + j over the destination list `row_nodes` (a < n_dst; entries < 0 are padding), edge slot e = row_nodes[a] * k + j.
@@ -270,16 +185,10 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
                    const unsigned char* __restrict__ tab_image, float coeff, const float* __restrict__ qnode, float* __restrict__ out, int out_by_slot, AggArgs agg, const __grid_constant__ LnParams lp) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t sbase = smem_u32(smem_raw);
-  const uint32_t sW = sbase + oW, sG = sbase + oG, sT = sbase + oT, sS = sbase + oS, sX = sbase + oX, sBar = sbase + oBar;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem_raw + oBar + 16 * 8);
-  // the warp index is broadcast from lane 0 so that the compiler KNOWS it is warp-uniform: role branches become uniform branches and
-  // every constant-bank read indexed by it (LayerNorm parameters, biases) goes through the uniform datapath (LDCU + UR operands)
-  // instead of per-thread LDC into vector registers
-#ifdef TDIFF_PLAIN_WARP_INDEX          // A/B switch (tools/build_variant.sh): the pre-change form, per-thread LDC
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-#else
+  const uint32_t sW = sbase + oW, sG = sbase + oG, sT = sbase + oT, sA = sbase + oA, sDp = sbase + oDp, sD = sbase + oD, sX = sbase + oX,
+                 sBar = sbase + oBar;
+  // the warp index is broadcast from lane 0 so that the compiler knows it is warp-uniform (role branches are uniform branches)
   const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-#endif
   auto bar = [&](int i) { return sBar + 8u * (uint32_t)i; };
   // row -> (destination slot, neighbour slot): k is a power of two for every shipped configuration but 48
   const int kshift = (k & (k - 1)) == 0 ? __ffs(k) - 1 : -1;
@@ -292,58 +201,46 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   if ((sbase & 1023u) != 0) __trap();            // SWIZZLE_128B atoms need a 1024-byte aligned window
   if (d_counts) { n_dst = d_counts[0]; split_dst = d_counts[1]; }      // destination subset compacted on the device
   const long long n_rows = n_dst * k, split_rows = split_dst * k;      // both multiples of 128 by construction of the lists
-  const long long n_tiles = (n_rows + 127) / 128;
+  const long long n_tiles = (n_rows + kTile - 1) / kTile;
   const long long my_tiles = (n_tiles > blockIdx.x) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-  auto tile_class = [&](long long t) -> int { return ((long long)(blockIdx.x + t * (long long)gridDim.x) * 128 >= split_rows) ? 1 : 0; };
+  auto tile_class = [&](long long t) -> int { return ((long long)(blockIdx.x + t * (long long)gridDim.x) * kTile >= split_rows) ? 1 : 0; };
 
-  // ---- one-time setup: weight image and the first tile's class table -> smem, barriers, TMEM
+  // ---- one-time setup: weight image and the first tile's class table -> smem (TMA bulk copies), barriers
   constexpr int kWAtom = NOUT * 128;            // one K-half of a weight piece: NOUT rows x 128 B
   constexpr int kWPiece = 2 * kWAtom;
-  constexpr uint32_t kIdescMain = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NOUT >> 3) << 17) | ((128u >> 4) << 24);
   if (tid == 0) {
     mbar_init(bar(B_LOAD), 1);
     mbar_init(bar(B_TAB), 1);
-    mbar_init(bar(B_S_FULL), kGatherWarps);
-    mbar_init(bar(B_S_EMPTY), kRowWarps);
     mbar_init(bar(B_G_FULL), kRowWarps);
+    mbar_init(bar(B_DPRE_FULL), kMmaWarps);
     mbar_init(bar(B_A_FULL), kRowWarps);
-    mbar_init(bar(B_A_EMPTY), 1);
-    mbar_init(bar(B_DPRE_FULL), 1);
-    mbar_init(bar(B_D_FULL0), 1);
-    mbar_init(bar(B_D_FULL1), 1);
-    mbar_init(bar(B_D_EMPTY0), kEpiWarps);
-    mbar_init(bar(B_D_EMPTY1), kEpiWarps);
+    mbar_init(bar(B_A_EMPTY), kMmaWarps);
+    mbar_init(bar(B_D_FULL), kMmaWarps);
+    mbar_init(bar(B_D_EMPTY), kEpiWarps);
     fence_barrier_init();
-    // the two MMA B operands arrive as TMA bulk copies (no registers, no per-thread loops); only the MMA-issuing warp waits for them
     mbar_expect_tx(bar(B_LOAD), 2u * kWPiece + (uint32_t)kTabClassBytes);
     bulk_g2s(sW, w2_image, 2u * kWPiece, bar(B_LOAD));
     bulk_g2s(sT, tab_image + (size_t)tile_class(0) * kTabClassBytes, (uint32_t)kTabClassBytes, bar(B_LOAD));
   }
-  if (warp == kMmaWarp) tmem_alloc(smem_u32(s_tmem), 512);
-  fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
   if (warp >= kRowWarp0) {
     // ================================================================= row threads (thread = edge row x 32 features)
-    reg_inc<80>();
-    const int rwp = warp - kRowWarp0, q = rwp & 3, qq = rwp >> 2;
-    const int r = 32 * q + lane;                    // row of the tile == TMEM lane
+    const int rwp = warp - kRowWarp0, q = rwp & 1, qq = rwp >> 1;
+    const int r = 32 * q + lane;                    // row of the tile
     float mu[5];
 #pragma unroll
     for (int i = 0; i < 5; ++i) mu[i] = lp.mu[5 * qq + i];
     const float coeff2 = coeff * 1.4426950408889634f;
-    const uint32_t s_row = sS + (uint32_t)qq * kSAtom + (uint32_t)r * kSRow;
     const uint32_t g_row = sG + (uint32_t)r * 128u;
-    const uint32_t xslot = sX + (uint32_t)r * 4u;          // exchange slots of this row: set 0 (sums) / set 1 at +2048, quarter qq at + qq*512
-    const uint32_t t_lane = tmem_base + ((uint32_t)(32 * q) << 16);
+    const uint32_t dp_row = sDp + 4u * ((uint32_t)r * kDRow + 32u * (uint32_t)qq);
+    const uint32_t a_row = sA + (uint32_t)(qq >> 1) * kGAtom + (uint32_t)r * 128u;     // K-half qq / 2 of piece 0; piece 1 at + 2 kGAtom
+    const uint32_t xslot = sX + (uint32_t)r * 4u;          // exchange slots of this row: set 0 (sums) / set 1 at +1024, quarter qq at + qq*256
     // metadata of this thread's row in tile `t` (s < 0: absent edge / padding destination / beyond the end)
     auto load_md = [&](long long t, int& s_, int& ty_, int& dst_, float& dist_) {
       s_ = -1; ty_ = 3; dst_ = 0; dist_ = 0.f;
       if (t < my_tiles) {
-        const long long idx = (blockIdx.x + t * (long long)gridDim.x) * 128 + r;
+        const long long idx = (blockIdx.x + t * (long long)gridDim.x) * kTile + r;
         if (idx < n_rows) {
           int j;
           const unsigned a = row_dst(idx, j);
@@ -376,9 +273,9 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       const uint32_t sw = (uint32_t)(r & 7);
       const uint32_t a_own = g_row + ((((uint32_t)qq + half) ^ sw) << 4), a_other = g_row + ((((uint32_t)qq + (half ^ 4u)) ^ sw) << 4);
       sts128(a_own, hi[0], hi[1], hi[2], hi[3]);
-      sts128(a_own + kAtom, lo[0], lo[1], lo[2], lo[3]);
+      sts128(a_own + kGAtom, lo[0], lo[1], lo[2], lo[3]);
       sts128(a_other, 0u, 0u, 0u, 0u);
-      sts128(a_other + kAtom, 0u, 0u, 0u, 0u);
+      sts128(a_other + kGAtom, 0u, 0u, 0u, 0u);
       fence_proxy_async();
       __syncwarp();
       if (lane == 0) mbar_arrive(bar(B_G_FULL));
@@ -388,59 +285,38 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
     load_md(0, s0, t0, d0, dist0);
     if (my_tiles > 0) write_g(s0, t0, dist0);
     load_md(1, s1, t1, d1, dist1);
-    WS_DECL(rs); WS_DECL(rd); WS_DECL(ra); WS_DECL(rt);
-#ifdef TDIFF_WAIT_STATS
-    const unsigned ws_loop0 = (unsigned)clock();
-#endif
     for (long long it = 0; it < my_tiles; ++it) {
       const uint32_t ph = (uint32_t)(it & 1);
       const bool valid = s0 >= 0;
-      // ---- P[dst, offA + 32*qq ..] (rows of a warp usually share the destination: broadcast loads) stays in flight while we wait
-      //      for the gathered source row in the staging tile
-      float4 av[8];
+      // ---- P[src, offB + 32*qq ..] (absent slots read the all-zero row `zero_row` kept by the engine) + P[dst, offA + 32*qq ..]
+      //      (rows of a warp usually share the destination: broadcast loads); both stay in flight while we wait for Dpre
+      const float* ps = P + (size_t)(valid ? s0 : zero_row) * TD_NPROJ + offB + 32 * qq;
+      float4 av[8], bv[8];
 #pragma unroll
       for (int c = 0; c < 8; ++c) {
+        bv[c] = __ldg(reinterpret_cast<const float4*>(ps + 4 * c));
         av[c] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (valid) av[c] = __ldg(reinterpret_cast<const float4*>(P + (size_t)d0 * TD_NPROJ + offA + 32 * qq + 4 * c));
       }
       f2 x[16];
-#ifdef TDIFF_ROW_SLEEP           // A/B switch: back off while waiting for the gather warps instead of spinning beside them
-      { WS_T0();
-        while (true) {
-          uint32_t done;
-          asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                       : "=r"(done) : "r"(bar(B_S_FULL)), "r"(ph) : "memory");
-          if (done) break;
-          __nanosleep(32);
-        }
-        WS_ADD(rs); }
-#else
-      { WS_T0(); mbar_wait(bar(B_S_FULL), ph); WS_ADD(rs); }
-#endif
 #pragma unroll
       for (int c = 0; c < 8; ++c) {
-        const float4 v = lds128(s_row + 16u * c);
-        x[2 * c] = add2(pk2(v.x, v.y), pk2(av[c].x, av[c].y)); x[2 * c + 1] = add2(pk2(v.z, v.w), pk2(av[c].z, av[c].w));
+        x[2 * c] = add2(pk2(bv[c].x, bv[c].y), pk2(av[c].x, av[c].y)); x[2 * c + 1] = add2(pk2(bv[c].z, bv[c].w), pk2(av[c].z, av[c].w));
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar(B_S_EMPTY));
       // ---- + gaussian/type block from the tensor core
-      { WS_T0(); mbar_wait(bar(B_DPRE_FULL), ph); WS_ADD(rd); }
-      tc_fence_after();
+      mbar_wait(bar(B_DPRE_FULL), ph);
       {
         uint32_t v0[16], v1[16];
-        const uint32_t ta = t_lane + kColDpre + (uint32_t)(32 * qq);
-        tmem_ld16_nowait(ta, v0);
-        tmem_ld16_nowait(ta + 16u, v1);
-        tmem_ld_wait();
+        lds16(dp_row, v0);
+        lds16(dp_row + 64u, v1);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           x[i] = add2(x[i], pk2(__uint_as_float(v0[2 * i]), __uint_as_float(v0[2 * i + 1])));
           x[8 + i] = add2(x[8 + i], pk2(__uint_as_float(v1[2 * i]), __uint_as_float(v1[2 * i + 1])));
         }
       }
-      tc_fence_before();
-      // ---- gaussians of the NEXT tile now (the small MMA and its round trip overlap this tile's LayerNorm), metadata two ahead
+      // ---- gaussians of the NEXT tile now (the small MMA overlaps this tile's LayerNorm), metadata two ahead.  Writing G(it+1)
+      //      also tells the MMA warpgroup that this warp has read Dpre(it).
       if (it + 1 < my_tiles) write_g(s1, t1, dist1);
       s0 = s1; t0 = t1; d0 = d1; dist0 = dist1;
       load_md(it + 2, s1, t1, d1, dist1);
@@ -451,9 +327,9 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       sa = add2(sa, add2(x[8], x[9])); sb = add2(sb, add2(x[10], x[11])); sc = add2(sc, add2(x[12], x[13])); sd = add2(sd, add2(x[14], x[15]));
       float p0, p1;
       upk2(add2(add2(sa, sb), add2(sc, sd)), p0, p1);
-      sts32f(xslot + (uint32_t)qq * 512u, p0 + p1);
+      sts32f(xslot + (uint32_t)qq * 256u, p0 + p1);
       named_bar_sync(1 + q, 128);
-      const float mean = ((lds32f(xslot) + lds32f(xslot + 512u)) + (lds32f(xslot + 1024u) + lds32f(xslot + 1536u))) * (1.0f / 128.0f);
+      const float mean = ((lds32f(xslot) + lds32f(xslot + 256u)) + (lds32f(xslot + 512u) + lds32f(xslot + 768u))) * (1.0f / 128.0f);
       const f2 mean2 = pk2(mean, mean);
       f2 qa = pk2(0.f, 0.f), qb = qa, qc = qa, qd = qa;
 #pragma unroll
@@ -462,11 +338,11 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
         qa = fma2(x[i], x[i], qa); qb = fma2(x[i + 1], x[i + 1], qb); qc = fma2(x[i + 2], x[i + 2], qc); qd = fma2(x[i + 3], x[i + 3], qd);
       }
       upk2(add2(add2(qa, qb), add2(qc, qd)), p0, p1);
-      sts32f(xslot + 2048u + (uint32_t)qq * 512u, p0 + p1);
+      sts32f(xslot + 1024u + (uint32_t)qq * 256u, p0 + p1);
       named_bar_sync(1 + q, 128);
-      const float var = ((lds32f(xslot + 2048u) + lds32f(xslot + 2560u)) + (lds32f(xslot + 3072u) + lds32f(xslot + 3584u))) * (1.0f / 128.0f);
+      const float var = ((lds32f(xslot + 1024u) + lds32f(xslot + 1280u)) + (lds32f(xslot + 1536u) + lds32f(xslot + 1792u))) * (1.0f / 128.0f);
       const float rstd = rsqrtf(var + 1e-5f);
-      // ---- affine + ReLU, bf16 split -> this row's 32 features of both A pieces (16 packed columns each) in tensor memory.
+      // ---- affine + ReLU, bf16 split -> this row's 32 features of both A pieces (K-major SWIZZLE_128B: 4 chunks of 16 B).
       //      Absent rows carry x = 0: their (finite) outputs are never consumed.
       uint32_t hi[16], lo[16];
       {
@@ -481,177 +357,94 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
           split2(fmaxf(y2, 0.f), fmaxf(y3, 0.f), hi[2 * c + 1], lo[2 * c + 1]);
         }
       }
-      { WS_T0(); mbar_wait(bar(B_A_EMPTY), ph ^ 1u); WS_ADD(ra); }         // the previous tile's MMAs have read A
-      tc_fence_after();
-      tmem_st16(t_lane + kColA + (uint32_t)(16 * qq), hi);
-      tmem_st16(t_lane + kColA + 64u + (uint32_t)(16 * qq), lo);
-      tmem_st_wait();
-      tc_fence_before();
+      mbar_wait(bar(B_A_EMPTY), ph ^ 1u);         // the previous tile's MMAs have read A
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const uint32_t a = a_row + ((((uint32_t)(4 * (qq & 1) + c)) ^ (uint32_t)(r & 7)) << 4);
+        sts128(a, hi[4 * c], hi[4 * c + 1], hi[4 * c + 2], hi[4 * c + 3]);
+        sts128(a + 2u * kGAtom, lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]);
+      }
+      fence_proxy_async();                        // A -> visible to the tensor-core (async) proxy
       __syncwarp();
       if (lane == 0) mbar_arrive(bar(B_A_FULL));
     }
-#ifdef TDIFF_WAIT_STATS
-    ws_rt = (unsigned)clock() - ws_loop0;
-    WS_FLUSH(0, rt); WS_FLUSH(1, rs); WS_FLUSH(2, rd); WS_FLUSH(3, ra);
-    if (lane == 0) atomicAdd(&g_wait_stats[11], 1ull);
-#endif
-  } else if (warp >= kGatherWarp0) {
-    // ================================================================= gather warps (lane = 4 features), 32 rows each; the last one
-    //                                                                   also issues the MMAs (one thread) between its copies
-    // Register budget.  The CTA is launched with 72 registers x 896 threads; setmaxnreg only moves registers INSIDE that allocation:
-    // the gather warps release (72 - 40) x 128 = 4096, exactly what the row warps' increase (80 - 72) x 512 needs (a smaller release
-    // leaves the row warps blocked in setmaxnreg.inc forever).  Local-memory spills are poison here (18 KB of L1 beside 209 KB of
-    // shared memory): measured on B200, variants of this loop with 100+ bytes of spills ran 15-20 % slower than this one (8 bytes).
-    reg_dec<40>();
-    const int gw = warp - kGatherWarp0;
-    const bool mma_warp = warp == kMmaWarp;
-    const int atom = lane >> 3, ch = lane & 7;
+  } else if (warp < kMmaWarps) {
+    // ================================================================= MMA warpgroup
     int cur_class = tile_class(0);
-    // source node of row 32*gw + lane of tile t
-    auto load_md = [&](long long t) -> int {
-      int s_ = -1;
-      if (t < my_tiles) {
-        const long long idx = (blockIdx.x + t * (long long)gridDim.x) * 128 + 32 * gw + lane;
-        if (idx < n_rows) {
-          int j;
-          const unsigned a = row_dst(idx, j);
-          const int dst = row_nodes[a];
-          if (dst >= 0) s_ = src[(size_t)dst * k + j];
-        }
-      }
-      return s_;
-    };
-    // Dpre = G(t) . TabClass^T   (K = 64: four K=16 instructions per product term)
-    WS_DECL(gs); WS_DECL(gc); WS_DECL(gg); WS_DECL(gm); WS_DECL(gt);
-    auto issue_pre = [&](long long t) {
-      { WS_T0(); mbar_wait(bar(B_G_FULL), (uint32_t)(t & 1)); WS_ADD(gg); }       // every row warp has written G(t), i.e. has also read Dpre(t-1): sT is idle
-      tc_fence_after();
+    for (long long t = 0; t < my_tiles; ++t) {
+      const uint32_t ph = (uint32_t)(t & 1);
+      // ---- Dpre = G(t) . TabClass^T   (K = 64: four K=16 instructions per product term)
+      mbar_wait(bar(B_G_FULL), ph);               // every row warp has written G(t), i.e. has also read Dpre(t-1)
+      if (t == 0) mbar_wait(bar(B_LOAD), 0);      // W2 pieces and the first class table have landed
       const int cls = tile_class(t);
-      if (t == 0) mbar_wait(bar(B_LOAD), 0);              // W2 pieces and the first class table have landed
-      if (cls != cur_class) {                            // at most once per CTA and launch (tiles are class-sorted): swap the table by TMA
-        if (lane == 0) {
+      if (cls != cur_class) {                     // at most once per CTA and launch (tiles are class-sorted): swap the table by TMA
+        if (tid == 0) {
           mbar_expect_tx(bar(B_TAB), (uint32_t)kTabClassBytes);
           bulk_g2s(sT, tab_image + (size_t)cls * kTabClassBytes, (uint32_t)kTabClassBytes, bar(B_TAB));
         }
         mbar_wait(bar(B_TAB), 0);
         cur_class = cls;
-        __syncwarp();
       }
-      if (MMA_LANE) {
-        const uint32_t d_addr = tmem_base + kColDpre;
+      {
+        float d[64];
+        wgmma_fence();
         uint32_t accum = 0;
 #pragma unroll
         for (int term = 0; term < 3; ++term) {
           const int pa_ = (term == 2) ? 1 : 0, pb_ = (term == 1) ? 1 : 0;      // a1b1, a1b2, a2b1
 #pragma unroll
           for (int kk = 0; kk < 4; ++kk) {
-            umma_ss(d_addr, desc_sw128(sG + pa_ * kAtom + kk * 32), desc_sw128(sT + pb_ * kAtom + kk * 32), kIdesc128, accum);
+            wgmma_n128(d, gmma_desc_sw128(sG + pa_ * kGAtom + kk * 32), gmma_desc_sw128(sT + pb_ * (kTabClassBytes / 2) + kk * 32), accum);
             accum = 1;
           }
         }
-        umma_commit(bar(B_DPRE_FULL));
+        wgmma_commit();
+        wgmma_wait_all();
+        store_frag<128>(sDp, d, warp, lane);
       }
       __syncwarp();
-    };
-    // D[t&1] = A(t) . W2^T, A pieces in tensor memory
-    auto issue_main = [&](long long t) {
-      const uint32_t ph = (uint32_t)(t & 1), ph2 = (uint32_t)((t >> 1) & 1);
-      { WS_T0(); mbar_wait_relaxed(bar(B_D_EMPTY0 + (int)ph), ph2 ^ 1u);
-        mbar_wait(bar(B_A_FULL), ph); WS_ADD(gm); }
-      tc_fence_after();
-      if (MMA_LANE) {
-        const uint32_t d_addr = tmem_base + kColD + ph * 128u;
+      if (lane == 0) mbar_arrive(bar(B_DPRE_FULL));
+      // ---- D = A(t) . W2^T
+      mbar_wait(bar(B_A_FULL), ph);
+      {
+        float d[NOUT / 2];
+        wgmma_fence();
         uint32_t accum = 0;
 #pragma unroll
         for (int term = 0; term < 3; ++term) {
           const int pa_ = (term == 2) ? 1 : 0, pb_ = (term == 1) ? 1 : 0;
 #pragma unroll
           for (int kk = 0; kk < 8; ++kk) {
-            const uint32_t woff = (kk >> 2) * kWAtom + (kk & 3) * 32;
-            umma_ts(d_addr, tmem_base + kColA + (uint32_t)pa_ * 64u + (uint32_t)kk * 8u, desc_sw128(sW + pb_ * kWPiece + woff), kIdescMain, accum);
+            const uint32_t aoff = (uint32_t)(pa_ * 2 * kGAtom + (kk >> 2) * kGAtom + (kk & 3) * 32);
+            const uint32_t woff = (uint32_t)(pb_ * kWPiece + (kk >> 2) * kWAtom + (kk & 3) * 32);
+            if constexpr (NOUT == 128) wgmma_n128(d, gmma_desc_sw128(sA + aoff), gmma_desc_sw128(sW + woff), accum);
+            else wgmma_n16(d, gmma_desc_sw128(sA + aoff), gmma_desc_sw128(sW + woff), accum);
             accum = 1;
           }
         }
-        umma_commit(bar(B_A_EMPTY));
-        umma_commit(bar(B_D_FULL0 + (int)ph));
+        wgmma_commit();
+        wgmma_wait_all();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar(B_A_EMPTY));
+        mbar_wait(bar(B_D_EMPTY), ph ^ 1u);       // the epilogue is done with D(t-1)
+        store_frag<NOUT>(sD, d, warp, lane);
       }
       __syncwarp();
-    };
-    int s0 = load_md(0);
-#ifdef TDIFF_WAIT_STATS
-    const unsigned ws_loop0 = (unsigned)clock();
-#endif
-    // iteration `it`: copy S(it) (overlaps the row threads' work on tile it-1), then Dpre(it), then the main MMA of tile it-1
-    for (long long it = 0; it <= my_tiles; ++it) {
-      if (it < my_tiles) {
-        const int s1 = load_md(it + 1);                      // next tile's metadata lands while this tile's rows are copied
-#ifdef TDIFF_PRE_FIRST          // A/B switch (measured: no gain): the small MMA before this warp's copies instead of after them
-        if (mma_warp) issue_pre(it);
-#endif
-        { WS_T0(); mbar_wait(bar(B_S_EMPTY), (uint32_t)((it & 1) ^ 1)); WS_ADD(gs); }
-#ifdef TDIFF_WAIT_STATS
-        const unsigned ws_copy0 = (unsigned)clock();
-#endif
-        // ---- P[src_row, offB + 4*lane ..] -> S, 32 rows x 512 B per warp, asynchronously (no registers, L2 -> shared)
-#ifndef TDIFF_BRANCHY_GATHER
-        // absent neighbour slots read the all-zero row `zero_row` of P (kept by the engine): no per-row predicate or zero store, and the
-        // fully unrolled loop shuffles with constant lane numbers -- 6 instead of 9 issue slots per row for the warp the row threads wait on
-        {
-          const unsigned sg = (unsigned)(s0 >= 0 ? s0 : zero_row);
-          const float* pl = P + offB + 4 * lane;
-          const uint32_t dst0 = sS + (uint32_t)atom * kSAtom + (uint32_t)(32 * gw) * kSRow + (uint32_t)(ch << 4);
-#pragma unroll
-          for (int rr = 0; rr < 32; ++rr) {
-            const unsigned sr = __shfl_sync(0xffffffffu, sg, rr);
-            cp_async16(dst0 + (uint32_t)rr * kSRow, pl + (size_t)sr * TD_NPROJ);
-          }
-        }
-#else                      // A/B switch: the per-row branch form measured before this change
-#pragma unroll 8
-        for (int rr = 0; rr < 32; ++rr) {
-          const int row = 32 * gw + rr;
-          const int sr = __shfl_sync(0xffffffffu, s0, rr);
-          const uint32_t dsta = sS + (uint32_t)atom * kSAtom + (uint32_t)row * kSRow + (uint32_t)(ch << 4);
-          if (sr >= 0) cp_async16(dsta, P + (size_t)sr * TD_NPROJ + offB + 4 * lane);
-          else sts128f(dsta, make_float4(0.f, 0.f, 0.f, 0.f));
-        }
-#endif
-        cp_async_wait_all();
-        __syncwarp();
-#ifdef TDIFF_WAIT_STATS
-        ws_gc += (unsigned)clock() - ws_copy0;
-#endif
-        if (lane == 0) mbar_arrive(bar(B_S_FULL));
-        s0 = s1;
-#ifndef TDIFF_PRE_FIRST
-        if (mma_warp) issue_pre(it);
-#endif
-      }
-      if (mma_warp && it >= 1) issue_main(it - 1);
+      if (lane == 0) mbar_arrive(bar(B_D_FULL));
     }
-#ifdef TDIFF_WAIT_STATS
-    ws_gt = (unsigned)clock() - ws_loop0;
-    WS_FLUSH(4, gt); WS_FLUSH(5, gs); WS_FLUSH(6, gc); WS_FLUSH(7, gg); WS_FLUSH(8, gm);
-    if (lane == 0) atomicAdd(&g_wait_stats[12], 1ull);
-    if (mma_warp) { WS_FLUSH(14, gt); WS_FLUSH(15, gs); }
-#endif
   } else {
-    // ================================================================= epilogue: warp w <-> TMEM lanes 32 (w%4) .., columns 64 (w/4) ..
-    const int eq = warp & 3;
-    const int HALF = warp >> 2;                    // one code copy for both column halves (b2 through indexed constant loads)
-    WS_DECL(ed); WS_DECL(et);
-#ifdef TDIFF_WAIT_STATS
-    const unsigned ws_loop0 = (unsigned)clock();
-#endif
+    // ================================================================= epilogue: warp 4+w <-> rows 32 (w%2) .., columns 64 (w/2) ..
+    const int eq = (warp - kEpiWarp0) & 1;
+    const int HALF = (warp - kEpiWarp0) >> 1;      // one code copy for both column halves (b2 through indexed constant loads)
+    const uint32_t drow = sD + 4u * ((uint32_t)(eq * 32 + lane) * kDRow + (uint32_t)(64 * HALF));
     for (long long it = 0; it < my_tiles; ++it) {
       const long long tile = blockIdx.x + it * gridDim.x;
-      const uint32_t ph = (uint32_t)(it & 1), ph2 = (uint32_t)((it >> 1) & 1);
-      const uint32_t tbase = tmem_base + ((uint32_t)(eq * 32) << 16) + kColD + ph * 128u + (uint32_t)(64 * HALF);
+      const uint32_t ph = (uint32_t)(it & 1);
       // fused aggregation (value launch, k == 32): everything that does not depend on the accumulator is fetched before waiting for it
       const bool do_agg = NOUT == 128 && qnode == nullptr && agg.logits != nullptr;
       const bool key_sm = NOUT == 128 && qnode != nullptr && agg.key_softmax;    // key launch, k == 32: softmax in this epilogue
-      const long long idx = tile * 128 + eq * 32 + lane;
-      const long long dslot = tile * 4 + eq;                          // k == 32: destination index of this warp's 32 rows
+      const long long idx = tile * kTile + eq * 32 + lane;
+      const long long dslot = tile * 2 + eq;                          // k == 32: destination index of this warp's 32 rows
       const int dnode = (do_agg && dslot < n_dst) ? row_nodes[dslot] : -1;
       const bool active = dnode >= 0;                                 // warp-uniform
       float w[8], hin[4], ew = 0.f;
@@ -672,9 +465,9 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
 #pragma unroll
         for (int j = 0; j < 4; ++j) hin[j] = (active && lane < 16) ? agg.h[(size_t)dnode * TD_H + 64 * HALF + 16 * j + lane] : 0.0f;
         // next tile: weights and destination row -> L1
-        const long long nslot = dslot + 4 * (long long)gridDim.x;
+        const long long nslot = dslot + 2 * (long long)gridDim.x;
         if (it + 1 < my_tiles && nslot < n_dst) {
-          prefetch_l1(agg.logits + (size_t)(idx + 128 * (long long)gridDim.x) * TD_HEADS + 8 * HALF);
+          prefetch_l1(agg.logits + (size_t)(idx + kTile * (long long)gridDim.x) * TD_HEADS + 8 * HALF);
           const int nn = row_nodes[nslot];
           if (lane < 2 && nn >= 0) prefetch_l1(agg.h + (size_t)nn * TD_H + 64 * HALF + 32 * lane);
         }
@@ -689,7 +482,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
           }
         }
         // key launches: next tile's query half row (2 lines per destination; the 32 rows of a warp share it when k == 32) -> L1
-        const long long nidx = idx + 128 * (long long)gridDim.x;
+        const long long nidx = idx + kTile * (long long)gridDim.x;
         if (NOUT == 128 && qnode != nullptr && it + 1 < my_tiles && nidx < n_rows && (lane & 15) == 0) {
           int j;
           const unsigned a = row_dst(nidx, j);
@@ -700,13 +493,12 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       // output row of the non-fused paths: the row index itself, or the edge slot (consumers that index by node * k + j)
       const long long orow = out_by_slot ? ((long long)dst * k + jj) : idx;
       const bool owrite = idx < n_rows && dst >= 0;
-      { WS_T0(); mbar_wait_relaxed(bar(B_D_FULL0 + (int)ph), ph2); WS_ADD(ed); }
-      tc_fence_after();
+      mbar_wait_relaxed(bar(B_D_FULL), ph);
       if (NOUT == 16) {
         // ---- xv: out[row, 0:16] = D[:, 0:16] + b2   (first column half only)
         if (HALF == 0) {
           uint32_t v[16];
-          tmem_ld16(tbase, v);
+          lds16(drow, v);
           if (owrite) {
             float* op = out + (size_t)orow * 16;
             stg256(op, __uint_as_float(v[0]) + lp.b2[0], __uint_as_float(v[1]) + lp.b2[1], __uint_as_float(v[2]) + lp.b2[2],
@@ -724,7 +516,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
           const int cb = 64 * HALF;
           const int c0 = 16 * j;
           uint32_t v[16];
-          tmem_ld16(tbase + (uint32_t)c0, v);
+          lds16(drow + 4u * (uint32_t)c0, v);
           float t[16];
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
@@ -741,7 +533,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
 #pragma unroll 1
         for (int c0 = 0; c0 < 64; c0 += 32) {
           uint32_t v[32];
-          tmem_ld32(tbase + (uint32_t)c0, v);
+          lds32(drow + 4u * (uint32_t)c0, v);
           if (owrite) {
 #pragma unroll
             for (int c = 0; c < 32; c += 8) {
@@ -763,22 +555,11 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
 #pragma unroll
           for (int i = 0; i < 4; ++i) qv[i] = __ldg(reinterpret_cast<const float4*>(qrow + c0 + 4 * i));
           uint32_t v[16];
-          tmem_ld16(tbase + (uint32_t)c0, v);
+          lds16(drow + 4u * (uint32_t)c0, v);
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
             const float* bb = lp.b2 + 64 * HALF + c0 + 8 * hh;
             const float4 qa = qv[2 * hh], qb = qv[2 * hh + 1];
-#ifdef TDIFF_PACKED_LOGITS        // A/B switch (measured -0.2 %, i.e. nothing: not shipped, its rounding order differs from the validated build)
-            // packed fp32 pairs: even and odd feature of the head accumulate separately (4 dependent FFMA2 instead of 8 dependent FFMA)
-            const uint32_t* vv = v + 8 * hh;
-            f2 acc = mul2(add2(pk2(__uint_as_float(vv[0]), __uint_as_float(vv[1])), pk2(bb[0], bb[1])), pk2(qa.x, qa.y));
-            acc = fma2(add2(pk2(__uint_as_float(vv[2]), __uint_as_float(vv[3])), pk2(bb[2], bb[3])), pk2(qa.z, qa.w), acc);
-            acc = fma2(add2(pk2(__uint_as_float(vv[4]), __uint_as_float(vv[5])), pk2(bb[4], bb[5])), pk2(qb.x, qb.y), acc);
-            acc = fma2(add2(pk2(__uint_as_float(vv[6]), __uint_as_float(vv[7])), pk2(bb[6], bb[7])), pk2(qb.z, qb.w), acc);
-            float s_even, s_odd;
-            upk2(acc, s_even, s_odd);
-            lg[c0 / 8 + hh] = (s_even + s_odd) * 0.35355339059327373f;          // 1/sqrt(8)
-#else
             float sacc = (__uint_as_float(v[8 * hh]) + bb[0]) * qa.x;
             sacc = fmaf(__uint_as_float(v[8 * hh + 1]) + bb[1], qa.y, sacc);
             sacc = fmaf(__uint_as_float(v[8 * hh + 2]) + bb[2], qa.z, sacc);
@@ -788,7 +569,6 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
             sacc = fmaf(__uint_as_float(v[8 * hh + 6]) + bb[6], qb.z, sacc);
             sacc = fmaf(__uint_as_float(v[8 * hh + 7]) + bb[7], qb.w, sacc);
             lg[c0 / 8 + hh] = sacc * 0.35355339059327373f;          // 1/sqrt(8)
-#endif
           }
         }
         if (key_sm) {
@@ -812,22 +592,9 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
         if (key_sm ? (idx < n_rows) : owrite)
           stg256(out + (size_t)(key_sm ? idx : orow) * TD_HEADS + 8 * HALF, lg[0], lg[1], lg[2], lg[3], lg[4], lg[5], lg[6], lg[7]);
       }
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(bar(B_D_EMPTY0 + (int)ph));
+      if (lane == 0) mbar_arrive(bar(B_D_EMPTY));
     }
-#ifdef TDIFF_WAIT_STATS
-    ws_et = (unsigned)clock() - ws_loop0;
-    WS_FLUSH(9, et); WS_FLUSH(10, ed);
-    if (lane == 0) atomicAdd(&g_wait_stats[13], 1ull);
-#endif
-  }
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -846,7 +613,7 @@ void td_launch_edge_mlp_v4(const float* P, int zero_row, const int* src, const u
   static size_t opted128[TD_MAX_DEVICES] = {0}, opted16[TD_MAX_DEVICES] = {0};
   td_opt_in_smem(edge_mlp_v4_kernel<128>, kSmem, opted128);
   td_opt_in_smem(edge_mlp_v4_kernel<16>, kSmem, opted16);
-  const long long n_tiles = (n_dst * k + 127) / 128;         // with d_counts: upper bound
+  const long long n_tiles = (n_dst * k + kTile - 1) / kTile;         // with d_counts: upper bound
   const int grid = (int)(n_tiles < sm_count ? n_tiles : sm_count);
   AggArgs agg = {agg_logits, agg_e_w, agg_h, (key_softmax && k == 32) ? 1 : 0};
   if (m.nout == 16)

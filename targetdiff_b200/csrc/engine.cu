@@ -62,13 +62,13 @@ struct EvPair { cudaEvent_t a, b; int kind; };
 
 struct tdiff_engine {
   tdiff_config cfg;
-  int device = 0, sm_count = 148;
+  int device = 0, sm_count = 132;
   // ---- weights (one device arena)
   float* arena = nullptr;
   std::vector<float> host_arena;        // host copy of the packed fp32 weights (kernel-argument constants are read from it)
   unsigned char* img_arena = nullptr;   // bf16-split second-layer weights in the tensor-core shared-memory image
-  int mlp_mode = 2;                     // 0: FP32 FFMA (edge_mlp.cu), 2: tcgen05 2-piece bf16 split / 3 products (default), 3: 3-piece / 6 products
-  bool mlp_v4 = true;                   // mode 2 edge MLPs: edge_mlp_v4.cu (both Linear layers + every edge type's gaussian block on tcgen05) instead of edge_mlp_tc.cu
+  int mlp_mode = 2;                     // 0: FP32 FFMA (edge_mlp.cu), 2: tensor-core (wgmma) 2-piece bf16 split / 3 products (default), 3: 3-piece / 6 products
+  bool mlp_v4 = true;                   // mode 2 edge MLPs: edge_mlp_v4.cu (both Linear layers + every edge type's gaussian block on the tensor cores) instead of edge_mlp_tc.cu
   std::vector<TdLayer> layers;
   const float *w_prot = nullptr, *b_prot = nullptr, *wl_t = nullptr, *bl = nullptr;
   const float *ew_w1t = nullptr, *ew_b1 = nullptr, *ew_g = nullptr, *ew_b = nullptr, *ew_w2 = nullptr, *ew_off = nullptr;
@@ -331,7 +331,7 @@ TdMlp mk_mlp(const float* base, const unsigned char* img_base, const MlpOff& o, 
 }  // namespace
 
 extern "C" const char* tdiff_last_error(void) { return g_err; }
-extern "C" const char* tdiff_version(void) { return "tdiff-b200 0.1 (sm_100a)"; }
+extern "C" const char* tdiff_version(void) { return "tdiff-b200 0.1 (sm_90a)"; }
 
 extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int n_entries, int device, tdiff_engine** out) {
   if (!cfg || !sd || !out) return set_err(TDIFF_EINVAL, "null argument");
@@ -361,7 +361,7 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
   CK(cudaSetDevice(device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major < 10) return set_err(TDIFF_ECUDA, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9) return set_err(TDIFF_ECUDA, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
 
   tdiff_engine* e = new tdiff_engine();
   e->cfg = *cfg; e->device = device; e->sm_count = prop.multiProcessorCount; e->K = e->KQ = cfg->knn; e->hybrid = cfg->cutoff_mode;
@@ -721,7 +721,7 @@ struct Prof {
 // per-edge MLP dispatch.  `list`: which destination set the launch covers.
 //   v4 (default): class-sorted destination lists; `qnode` != NULL marks a key MLP whose output is 16 attention logits (or, with
 //   `key_softmax`, softmax weights * e_w) per row; `agg_logits` / `agg_h` make the value launch perform the attention aggregation.
-//   earlier modes: tcgen05 second Linear with keys / values in HBM (edge_mlp_tc.cu) or the FP32 FFMA build (edge_mlp.cu).
+//   earlier modes: tensor-core second Linear with keys / values in HBM (edge_mlp_tc.cu) or the FP32 FFMA build (edge_mlp.cu).
 enum RowList { ROWS_ALL = 0, ROWS_LIGAND = 1, ROWS_RELEVANT = 2 };
 bool fused_logits(const tdiff_engine* e) { return e->mlp_mode == 2 && e->mlp_v4; }
 void edge_mlp(tdiff_engine* e, const float* P, const float4* xm, const int* src, const unsigned char* etype, RowList list, int K, const TdMlp& m,

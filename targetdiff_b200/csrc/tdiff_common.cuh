@@ -1,4 +1,4 @@
-// tdiff_common.cuh -- shared definitions for the sm_100a kernels of libtdiff.so.
+// tdiff_common.cuh -- shared definitions for the sm_90a kernels of libtdiff.so.
 //
 // Vocabulary follows the reference: nodes = protein + ligand atoms in `compose_context` order
 // (reference models/common.py:120-137), edges = dst-sorted k-NN slots (node i owns slots [i*K, (i+1)*K),

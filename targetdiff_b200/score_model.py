@@ -5,7 +5,7 @@ Mirrors the reference's Python surface (models/molopt_score_model.py:200-368,633
 15 schedule tables, so `load_state_dict(ckpt['model'])` is strict-compatible), `forward`, `sample_diffusion`, and the
 module-level `log_sample_categorical` / `center_pos` helpers that scripts/sample_diffusion.py imports.
 
-The modules below only *hold parameters*: every computation goes through libtdiff.so (hand-written sm_100a kernels,
+The modules below only *hold parameters*: every computation goes through libtdiff.so (hand-written sm_90a kernels,
 include/tdiff.h).  There is no PyTorch/CPU execution path; calling forward on CPU tensors raises.
 """
 import ctypes
@@ -286,7 +286,7 @@ class ScorePosNet3D(nn.Module):
         Returns {'pred_ligand_pos','pred_ligand_v','final_h','final_ligand_h'}; additionally 'edge_index' (int64 [2,E]) and, with
         `return_edge_weight`, 'edge_weight' [E]: the global edge gate e_w in edge_index order (models/uni_transformer.py:312-316)."""
         if return_all:
-            raise NotImplementedError('return_all=True (per-block outputs) is not implemented by the B200 engine')
+            raise NotImplementedError('return_all=True (per-block outputs) is not implemented by the H100 engine')
         dev = protein_pos.device
         eng = self.engine(dev)
         lib = _lib.load()
@@ -386,7 +386,7 @@ class ScorePosNet3D(nn.Module):
 
     # ------------------------------------------------------------------ out of scope on this path
     def get_diffusion_loss(self, *a, **k):
-        raise NotImplementedError('training is out of scope of the B200 sampling engine (SURVEY.md section 2)')
+        raise NotImplementedError('training is out of scope of the H100 sampling engine (SURVEY.md section 2)')
 
     # ------------------------------------------------------------------ second consumer of forward (SURVEY.md 8(f) n3)
     def _tab(self, name, t, batch):

@@ -1,4 +1,4 @@
-"""CUDA path (through the C-ABI of libtdiff.so) vs the CPU oracle -- run on the B200 box with `-m gpu`.
+"""CUDA path (through the C-ABI of libtdiff.so) vs the CPU oracle -- run on an H100 with `-m gpu`.
 
 Tolerances (BASELINE.json north_star): edge_index bit-exact; positions within 1e-4 relative; logits within 1e-3."""
 import os

@@ -5,8 +5,7 @@ center_pos_mode='none') against the live CPU oracle.  Run with -m gpu.
 
 Tolerances (BASELINE.json north_star): positions 1e-4 relative (atol 1e-4 A for near-zero coordinates), log-probabilities 1e-3,
 sampled atom types identical.  A free-running chain contains discrete decisions (k-NN membership, Gumbel arg-max), so each long
-test first reports where -- if anywhere -- the discrete trajectories part (profiles/r02_chain_parity_*.json is written from
-the same numbers by tools/chain_parity_report.py)."""
+test first reports where -- if anywhere -- the discrete trajectories part."""
 import json
 import os
 

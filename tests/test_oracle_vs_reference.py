@@ -1,36 +1,43 @@
-"""Pins oracle/restate.py against the UNMODIFIED reference (run under oracle/shims).  Build container only:
-skipped where /root/reference is absent (the GPU box) -- the committed tests/golden/ vectors carry the pin there."""
+"""Pins oracle/restate.py against the UNMODIFIED reference (run under oracle/shims): the restatement must reproduce, bit for bit,
+what the reference returned on the same inputs, stored in tests/golden/reference_pins.pt by oracle/make_reference_pins.py."""
+import os
+import sys
+
 import pytest
 import torch
 
+from oracle import make_reference_pins as pins_mod
 from oracle import refload, restate, synth
+from oracle.make_reference_pins import OPTION_CONFIGS, equal, option_id
 
-pytestmark = pytest.mark.skipif(not refload.reference_available(), reason='reference tree not present')
-
-
-@pytest.fixture(scope='module')
-def ref_model():
-    ref = refload.import_reference()
-    cfg = refload.default_model_config()
-    model = ref.ScorePosNet3D(cfg, synth.PROTEIN_FEATURE_DIM, synth.LIGAND_NUM_CLASSES).eval()
-    return ref, model
+if refload.SHIMS not in sys.path:           # torch_geometric / easydict stand-ins
+    sys.path.insert(0, refload.SHIMS)
 
 
-def test_state_dict_layout_matches_reference(ref_model):
-    _, model = ref_model
-    sd = model.state_dict()
+@pytest.fixture(scope='module', autouse=True)
+def pins():
+    n = torch.get_num_threads()
+    torch.set_num_threads(pins_mod.THREADS)       # the thread count the pins were computed with
+    yield torch.load(pins_mod.OUT, weights_only=True)
+    torch.set_num_threads(n)
+
+
+def test_state_dict_layout_matches_reference(pins):
     spec = synth.state_dict_spec()
-    assert list(sd.keys()) == [k for k, _, _ in spec]
-    for k, shape, _ in spec:
-        assert tuple(sd[k].shape) == tuple(shape), k
-    assert len(spec) == 384
+    assert equal([(k, tuple(shape)) for k, shape, _ in spec], pins['state_dict_layout'])
+    assert len(spec) == pins['state_dict_size'] == 384
 
 
-def test_schedules_bit_exact(ref_model):
-    _, model = ref_model
+def test_schedules_bit_exact(pins):
     sched = restate.make_schedules()
     for k in synth.SCHEDULE_KEYS:
-        assert torch.equal(model.state_dict()[k], sched[k]), k
+        assert equal(sched[k], pins['schedules'][k]), k
+
+
+def _assert_chain(got, want, keys=('pos_traj', 'v_traj', 'v0_traj', 'vt_traj')):
+    assert equal(got['pos'], want['pos']) and equal(got['v'], want['v'])
+    for k in keys:
+        assert equal(list(got[k]), want[k]), k
 
 
 def test_knn_shim_equals_canonical_restatement():
@@ -58,145 +65,98 @@ def test_knn_small_graph_and_ties():
     assert ((a[1] >= 5).sum()) == 40 * 32
 
 
-def test_forward_bit_exact(ref_model):
-    ref, model = ref_model
+def test_forward_bit_exact(pins):
+    want = pins['forward']
     sd = synth.make_state_dict(0, schedules=restate.make_schedules())
-    model.load_state_dict(sd, strict=True)
     b = synth.make_batch(1, 2, n_protein=60, ligand_sizes=[9, 7])
-    with torch.no_grad():
-        pp, lp, _ = ref.center_pos(b['protein_pos'], b['init_ligand_pos'], b['batch_protein'], b['batch_ligand'])
-        want = model(pp, b['protein_v'], b['batch_protein'], lp, b['init_ligand_v'], b['batch_ligand'])
     pp2, lp2, _ = restate.center_pos(b['protein_pos'], b['init_ligand_pos'], b['batch_protein'], b['batch_ligand'])
-    assert torch.equal(pp, pp2) and torch.equal(lp, lp2)
+    assert equal(pp2, want['protein_pos']) and equal(lp2, want['ligand_pos'])
     got = restate.forward(sd, None, pp2, b['protein_v'], b['batch_protein'], lp2, b['init_ligand_v'], b['batch_ligand'])
     for k in ('pred_ligand_pos', 'pred_ligand_v', 'final_h', 'final_ligand_h'):
-        assert torch.equal(want[k], got[k]), k
+        assert equal(got[k], want[k]), k
 
 
-def test_sampling_chain_bit_exact(ref_model):
-    _, model = ref_model
+def test_sampling_chain_bit_exact(pins):
     sd = synth.make_state_dict(3, schedules=restate.make_schedules())
-    model.load_state_dict(sd, strict=True)
     b = synth.make_batch(2, 2, n_protein=48, ligand_sizes=[8, 6])
     S = 3
     pn, vu = synth.make_tape(7, S, len(b['batch_ligand']))
     args = (b['protein_pos'], b['protein_v'], b['batch_protein'], b['init_ligand_pos'], b['init_ligand_v'], b['batch_ligand'])
-    with torch.no_grad(), refload.noise_tape(pn, vu):
-        want = model.sample_diffusion(*args, num_steps=S, center_pos_mode='protein')
     got = restate.sample_diffusion(sd, None, *args, pn, vu, num_steps=S)
-    assert torch.equal(want['pos'], got['pos']) and torch.equal(want['v'], got['v'])
-    for k in ('pos_traj', 'v_traj', 'v0_traj', 'vt_traj'):
-        assert all(torch.equal(a, c) for a, c in zip(want[k], got[k])), k
+    _assert_chain(got, pins['chain'])
 
 
 @pytest.mark.parametrize('steps', [[0, 999], [417, 3], None])
-def test_likelihood_estimation_matches_reference(ref_model, steps):
+def test_likelihood_estimation_matches_reference(pins, steps):
     """SURVEY 8(f) n3: the second consumer of `forward` (reference models/molopt_score_model.py:565-617), incl. the decoder
     branch (t = 0) and the prior branch (time_step == T)."""
-    _, model = ref_model
     sd = synth.make_state_dict(5, schedules=restate.make_schedules())
-    model.load_state_dict(sd, strict=True)
     b = synth.make_batch(4, 2, n_protein=52, ligand_sizes=[7, 10])
     Nl = len(b['batch_ligand'])
     pn, vu = synth.make_tape(9, 1, Nl)
     t = torch.tensor(steps) if steps is not None else torch.full((2,), 1000)
     args = (b['protein_pos'], b['protein_v'], b['batch_protein'], b['init_ligand_pos'], b['init_ligand_v'], b['batch_ligand'])
-    with torch.no_grad(), refload.noise_tape(pn, vu):
-        want = model.likelihood_estimation(*args, time_step=t)
+    want = pins['likelihood'][str(steps)]
     got = restate.likelihood_estimation(sd, None, *args, t, pn[0], vu[0])
     for w, g in zip(want, got):
         assert w.shape == g.shape == (2,)
         torch.testing.assert_close(g, w, rtol=1e-6, atol=1e-7)
 
 
-def test_sampling_chain_noise_mean_type_bit_exact():
+def test_sampling_chain_noise_mean_type_bit_exact(pins):
     """SURVEY 8(f) n2: model_mean_type='noise' (reference models/molopt_score_model.py:663-666, :419-422)."""
-    ref = refload.import_reference()
-    cfg = refload.default_model_config()
-    cfg.update({'model_mean_type': 'noise'})
-    model = ref.ScorePosNet3D(cfg, synth.PROTEIN_FEATURE_DIM, synth.LIGAND_NUM_CLASSES).eval()
     sd = synth.make_state_dict(6, schedules=restate.make_schedules())
-    model.load_state_dict(sd, strict=True)
     b = synth.make_batch(8, 2, n_protein=48, ligand_sizes=[8, 6])
     S = 3
     pn, vu = synth.make_tape(7, S, len(b['batch_ligand']))
     args = (b['protein_pos'], b['protein_v'], b['batch_protein'], b['init_ligand_pos'], b['init_ligand_v'], b['batch_ligand'])
-    with torch.no_grad(), refload.noise_tape(pn, vu):
-        want = model.sample_diffusion(*args, num_steps=S, center_pos_mode='protein')
     got = restate.sample_diffusion(sd, {'model_mean_type': 'noise'}, *args, pn, vu, num_steps=S)
-    assert torch.equal(want['pos'], got['pos']) and torch.equal(want['v'], got['v'])
-    for k in ('pos_traj', 'v_traj', 'v0_traj', 'vt_traj'):
-        assert all(torch.equal(a, c) for a, c in zip(want[k], got[k])), k
+    _assert_chain(got, pins['chain_noise'])
 
 
-OPTION_CONFIGS = [{'num_blocks': 2}, {'ew_net_type': 'r'}, {'ew_net_type': 'm'}, {'ew_net_type': 'none'}, {'x2h_out_fc': True},
-                  {'time_emb_dim': 1, 'time_emb_mode': 'simple'}, {'num_blocks': 2, 'ew_net_type': 'r', 'x2h_out_fc': True, 'time_emb_dim': 1},
-                  {'cutoff_mode': 'hybrid'}, {'cutoff_mode': 'hybrid', 'knn': 8, 'num_blocks': 2}]
-
-
-@pytest.mark.parametrize('cfgd', OPTION_CONFIGS, ids=lambda c: ','.join('%s=%s' % kv for kv in c.items()))
-def test_backbone_options_restatement_bit_exact(cfgd):
+@pytest.mark.parametrize('cfgd', OPTION_CONFIGS, ids=option_id)
+def test_backbone_options_restatement_bit_exact(pins, cfgd):
     """SURVEY 8(f) n2: num_blocks > 1, ew_net_type r / m / none, x2h_out_fc, time_emb_mode 'simple', cutoff_mode 'hybrid' -- state_dict layout (key order and
     shapes) and a 3-step sampling chain of the restatement against the unmodified reference, bit for bit."""
-    ref = refload.import_reference()
-    cfg = refload.default_model_config()
-    cfg.update(cfgd)
-    model = ref.ScorePosNet3D(cfg, synth.PROTEIN_FEATURE_DIM, synth.LIGAND_NUM_CLASSES).eval()
+    want = pins['options'][option_id(cfgd)]
     sd = synth.make_state_dict(0, cfgd, schedules=restate.make_schedules(cfgd))
-    assert list(model.state_dict().keys()) == list(sd.keys())
-    model.load_state_dict(sd, strict=True)
+    assert equal(list(sd.keys()), want['keys'])
     b = synth.make_batch(3, 2, n_protein=60, ligand_sizes=[9, 7])
     S = 3
     pn, vu = synth.make_tape(5, S, 16)
     args = (b['protein_pos'], b['protein_v'], b['batch_protein'], b['init_ligand_pos'], b['init_ligand_v'], b['batch_ligand'])
-    with torch.no_grad(), refload.noise_tape(pn, vu):
-        r = model.sample_diffusion(*args, num_steps=S, center_pos_mode='protein')
     w = restate.sample_diffusion(sd, cfgd, *args, pn, vu, num_steps=S)
-    assert torch.equal(r['pos'], w['pos']) and torch.equal(r['v'], w['v'])
-    for a, c in zip(r['v0_traj'] + r['vt_traj'] + r['pos_traj'], w['v0_traj'] + w['vt_traj'] + w['pos_traj']):
-        assert torch.equal(a, c)
+    _assert_chain(w, want, keys=('v0_traj', 'vt_traj', 'pos_traj'))
 
 
-def test_sampling_driver_restatement_bit_exact():
+def test_sampling_driver_restatement_bit_exact(pins):
     """a1: oracle.restate.sample_diffusion_ligand against the UNMODIFIED reference driver (scripts/sample_diffusion.py:31-116, imported with
     placeholders for rdkit / openbabel / lmdb) on the 1h36 pocket: same seeds -> the same prior sizes, positions, types and trajectories."""
     import json
-    import os
+    import random
     import numpy as np
-    sd_mod, sfp = refload.import_reference_scripts()
-    import utils.misc as misc
-    import utils.transforms as trans
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    data = trans.FeaturizeProteinAtom()(sfp.pdb_to_pocket_data(os.path.join(root, 'tests', 'golden', '1h36_pocket10.pdb')))
-    ref = refload.import_reference()
-    sd = synth.make_state_dict(0, schedules=restate.make_schedules())
-    model = ref.ScorePosNet3D(refload.default_model_config(), synth.PROTEIN_FEATURE_DIM, synth.LIGAND_NUM_CLASSES).eval()
-    model.load_state_dict(sd, strict=True)
-    misc.seed_all(2021)
-    out = sd_mod.sample_diffusion_ligand(model, data, 3, batch_size=2, device='cpu', num_steps=2, center_pos_mode='protein', sample_num_atoms='prior')
-    prior = json.load(open(os.path.join(root, 'targetdiff_b200', 'data', 'atom_num_prior.json')))
-    misc.seed_all(2021)
-    out2 = restate.sample_diffusion_ligand(sd, None, data.protein_pos, data.protein_atom_feature, 3, prior, batch_size=2, num_steps=2)
-    for a, b in zip(out[:6], out2[:6]):
-        assert len(a) == len(b) == 3 and all(np.array_equal(x, y) for x, y in zip(a, b))
-    # the product's PDB ingest gives the reference's tensors
     from targetdiff_b200.pocket import pdb_to_pocket_data
-    mine = pdb_to_pocket_data(os.path.join(root, 'tests', 'golden', '1h36_pocket10.pdb'))
-    assert torch.equal(mine.protein_pos, data.protein_pos) and torch.equal(mine.protein_atom_feature, data.protein_atom_feature)
+    want = pins['driver']
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    # the product's PDB ingest gives the reference's tensors
+    data = pdb_to_pocket_data(os.path.join(root, 'tests', 'golden', '1h36_pocket10.pdb'))
+    assert equal(data.protein_pos, want['protein_pos']) and equal(data.protein_atom_feature, want['protein_atom_feature'])
+    sd = synth.make_state_dict(0, schedules=restate.make_schedules())
+    prior = json.load(open(os.path.join(root, 'targetdiff_b200', 'data', 'atom_num_prior.json')))
+    # the reference driver's global seeding (utils/misc.py seed_all)
+    torch.manual_seed(2021)
+    np.random.seed(2021)
+    random.seed(2021)
+    out2 = restate.sample_diffusion_ligand(sd, None, data.protein_pos, data.protein_atom_feature, 3, prior, batch_size=2, num_steps=2)
+    for a, b in zip(want['outputs'], out2[:6]):
+        assert len(a) == len(b) == 3 and all(equal(torch.from_numpy(np.asarray(y)), x) for x, y in zip(a, b))
 
 
-def test_check_stability_restatement_equals_reference():
+def test_check_stability_restatement_equals_reference(pins):
     """n4: the bond-count stability screen (utils/evaluation/analyze.py:106-143) on random molecule-like point sets."""
     import numpy as np
-    refload.import_reference_scripts()          # installs the placeholders (matplotlib) the module imports at the top
-    import importlib
-    analyze = importlib.import_module('utils.evaluation.analyze')
-    rng = np.random.RandomState(0)
-    for n in (1, 2, 9, 25, 40):
-        for hs in (False, True):
-            pos = np.cumsum(rng.normal(scale=0.85, size=(n, 3)), axis=0)          # chain-like: neighbours at bonding distance
-            z = rng.choice([1, 6, 7, 8, 9, 15, 16, 17], size=n, p=[0.1, 0.5, 0.12, 0.15, 0.03, 0.02, 0.05, 0.03])
-            want = analyze.check_stability(pos, z, hs=hs, return_nr_bonds=True)
-            got = restate.check_stability(pos, z, hs=hs)
-            assert (bool(want[0]), want[1], want[2]) == (bool(got[0]), got[1], got[2])
-            assert np.array_equal(want[3], got[3])
+    assert len(pins['stability']) == 2 * len(pins_mod.STABILITY_SIZES)
+    for case in pins['stability']:
+        got = restate.check_stability(case['pos'].numpy(), case['z'].numpy(), hs=case['hs'])
+        assert [bool(got[0]), int(got[1]), int(got[2])] == case['result']
+        assert np.array_equal(case['nr_bonds'].numpy(), np.asarray(got[3]))

@@ -48,10 +48,10 @@ def test_ligand_class_maps():
     assert is_aromatic_from_index(idx) == [False, False, True, False, True, False, True, False, False, True, False, True, False]
 
 
-REF_PDB = '/root/reference/examples/1h36_A_rec_1h36_r88_lig_tt_docked_0_pocket10.pdb'
+# the reference's examples/1h36_A_rec_1h36_r88_lig_tt_docked_0_pocket10.pdb, byte for byte
+REF_PDB = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', '1h36_pocket10.pdb')
 
 
-@pytest.mark.skipif(not os.path.exists(REF_PDB), reason='reference examples/ not present')
 def test_1h36_pocket_matches_survey_facts():
     data = pdb_to_pocket_data(REF_PDB)
     el = data.protein_element.tolist()

@@ -3,7 +3,7 @@
 steps, pockets sharded over the GPUs of one box (scripts/batch_sample_diffusion.sh:15-21 assigns pocket i to worker i % 8).
 
     torchrun --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29511 tools/cfg4_sweep.py \
-        --pockets 100 --samples 100 --steps 1000 --schedule round_robin --out gpurun_out/r02_cfg4_round_robin.json
+        --pockets 100 --samples 100 --steps 1000 --schedule round_robin --out cfg4_round_robin.json
 
 Everything goes through the product's own command (targetdiff_b200.cli sample_pockets: checkpoint load on rank 0 + one NCCL weight
 broadcast, PDB ingest, size prior, sample_diffusion_ligand, result_{i}.pt files).  The pockets are synthetic (no dataset offline):

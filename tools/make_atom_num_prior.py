@@ -7,7 +7,7 @@ import importlib.util
 import json
 import os
 
-REF = os.environ.get('TARGETDIFF_REFERENCE', '/root/reference')
+REF = os.environ.get('TARGETDIFF_REFERENCE', '')
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'targetdiff_b200', 'data', 'atom_num_prior.json')
 
 spec = importlib.util.spec_from_file_location('atom_num_config', os.path.join(REF, 'utils', 'evaluation', 'atom_num_config.py'))

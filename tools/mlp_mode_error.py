@@ -1,4 +1,4 @@
-"""GPU: compare the three edge-MLP execution modes (FP32 FFMA, tcgen05 3-term, tcgen05 6-term) against the CPU oracle."""
+"""GPU: compare the three edge-MLP execution modes (FP32 FFMA, wgmma 3-term, wgmma 6-term) against the CPU oracle."""
 import os
 import sys
 import time

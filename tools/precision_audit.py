@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Precision audit of the engine's arithmetic modes over a FULL 1000-step free-running chain (run on a GPU box):
 
-    python tools/precision_audit.py [--out profiles/r02_precision_audit.json]
+    python tools/precision_audit.py [--out audit.json]
 
 For every golden chain the unmodified reference wrote (tests/golden/chain_1000_cfg1*.npz: default weights and a stressed variant with
 all Linear weights scaled up, a stand-in for the sharper attention of a trained checkpoint) and every edge-MLP execution mode
