@@ -171,16 +171,19 @@ void pack_umma_image(const float* w2, std::vector<unsigned char>& img, size_t of
 // Gaussian/type blocks as the B operand of the small "pre" MMA of edge_mlp_v4.cu: per destination class one table of
 // [128 out (N) x 64 K-slots] in two bf16 pieces, K-major SWIZZLE_128B (128-byte rows, 16-byte chunk index XOR row % 8).
 // Class 0 (protein destination): slots 0-31 = type 3 (P->P), 32-63 = type 1 (L->P); class 1 (ligand destination): type 2 (P->L) / type 0 (L->L).
-// Inside a 32-slot half: 8*c + i = gaussian 5*c + i (c < 4, i < 5), slot 29 = constant row (type column + bias), all other slots 0.
+// Inside a 32-slot half the slots follow the kernel's register A fragment: slot 8*c + 2*q + b is held by quad lane q, and the lane's
+// m = 2*c + b (m < 8) picks gaussian 5*q + m for m < 5, the constant row (type column + bias) for q = 3, m = 5, and 0 otherwise --
+// every lane of a quad evaluates 5 gaussians per row.
 void pack_tabcls_image(const float* tab /*[4][21][128]*/, std::vector<unsigned char>& img, size_t off) {
   static const int type_of[2][2] = {{3, 1}, {2, 0}};
   for (int cls = 0; cls < 2; ++cls)
     for (int n = 0; n < 128; ++n)
       for (int slot = 0; slot < 64; ++slot) {
         const int half = slot >> 5, sl = slot & 31;
+        const int q = (sl & 7) >> 1, m = 2 * (sl >> 3) + (sl & 1);
         int j = -1;
-        if ((sl & 7) < 5) j = 5 * (sl >> 3) + (sl & 7);
-        else if (sl == 29) j = 20;
+        if (m < 5) j = 5 * q + m;
+        else if (m == 5 && q == 3) j = 20;
         float r = j >= 0 ? tab[((size_t)type_of[cls][half] * TD_TAB + j) * TD_H + n] : 0.0f;
         const size_t o = (size_t)n * 128 + (size_t)(((slot >> 3) ^ (n & 7)) * 16) + (size_t)(slot & 7) * 2;
         for (int p = 0; p < 2; ++p) {
