@@ -16,11 +16,15 @@
 //   * the epilogues work on the D fragment; only the key softmax and the fused aggregation exchange per-warp partials through a
 //     small shared-memory slot between the two warps that hold one destination's 32 rows.
 //
-// CTA = kCons consumer warpgroups, one CTA per SM, persistent over tiles of 64 edge rows (one wgmma M); warpgroup c takes the CTA's
-// tiles c, c + kCons, ..., so one warpgroup's CUDA-core work (gathers, gaussians, LayerNorm, epilogue) overlaps another's MMAs.
-// P rows are gathered from L2 straight into the fragment registers.
-// Shared memory: W2 pieces 64 KB | both class tables 64 KB | LayerNorm affine + b2 1.5 KB | exchange slots 4 KB per warpgroup.
-// bf16 split: 2 pieces / 3 products (a1b1 + a1b2 + a2b1).
+// CTA = one producer warpgroup + kCons consumer warpgroups, one CTA per SM, persistent over tiles of 64 edge rows (one wgmma M).
+// The producer (one warp per consumer; `setmaxnreg` leaves it 40 registers and gives the consumers 232) stages each tile in shared
+// memory ahead of its consumer: the rows' metadata and the P[src] / P[dst] rows as 512-byte bulk copies.  Consumer c takes the CTA's tiles
+// c, c + kCons, ... and owns P stage c, which it hands back right after reading it (before the LayerNorm).  The two consumers'
+// tensor-core phases (pre-MMA, main MMA) run in a fixed alternating order (two named barriers): one consumer's MMAs are issued
+// whole while the other does its LayerNorm, split and epilogue, so the two never interleave on the tensor cores.
+// Shared memory: W2 pieces 64 KB | both class tables 64 KB | LayerNorm affine + b2 1.5 KB | exchange slots 4 KB per consumer |
+// 2 P stages of 39 KB (64 P[src] rows with a 544-byte stride, which makes the fragment-order reads free of bank conflicts,
+// kDst P[dst] rows, 64 metadata records) | mbarriers.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -31,12 +35,20 @@
 namespace v4 {
 
 constexpr int kCons = 2;                   // consumer warpgroups
-constexpr int kThreads = kCons * 128;
+constexpr int kThreads = (kCons + 1) * 128;  // warpgroup 0 is the producer
 constexpr int kTile = 64;                  // rows per tile
 constexpr int kTabClassBytes = 2 * 128 * 128;   // one class table: 2 bf16 pieces of [128 x 64]
+constexpr int kProdRegs = 40, kConsRegs = 232;  // setmaxnreg: 128 * 40 + 2 * 128 * 232 = 384 * 168 (the launch's allocation)
+// P stage: P[src] rows (stride padded by 32 B: the 8 rows one fragment load touches fall in distinct banks), the tile's first kDst
+// destinations' P[dst] rows (k >= 10 never needs more; rows of further destinations are read from global memory), and per row
+// the metadata record {node, src, dist, type | (dst slot + 1) << 8 | neighbour slot << 16}
+constexpr int kSrcStride = 512 + 32, kDst = 8;
+constexpr int sSrc = 0, sDstRows = sSrc + kTile * kSrcStride, sMeta = sDstRows + kDst * 512, kStage = sMeta + kTile * 16;
 // shared-memory map (bytes from the 1024-aligned base)
-constexpr int oW = 0, oT = oW + 4 * 128 * 128, oPar = oT + 2 * kTabClassBytes, oX = oPar + 3 * 128 * 4, oBar = oX + kCons * 4 * 2 * 128 * 4,
-              kSmem = oBar + 8;
+constexpr int oW = 0, oT = oW + 4 * 128 * 128, oPar = oT + 2 * kTabClassBytes, oX = oPar + 3 * 128 * 4, oStage = oX + kCons * 4 * 2 * 128 * 4,
+              oBar = oStage + kCons * kStage, kSmem = oBar + 8 * (1 + 2 * kCons);   // barriers: weights, full[kCons], empty[kCons]
+static_assert(oStage % 128 == 0 && kStage % 128 == 0 && kSmem <= 227 * 1024, "shared-memory map");
+constexpr int kOrderBar = 5;               // named barriers kOrderBar + c: consumer c may issue its next MMA phase (1-4: warp pairs)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -56,7 +68,14 @@ __device__ __forceinline__ void bulk_g2s(uint32_t smem_dst, const void* gsrc, ui
                "r"(bar) : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+__device__ __forceinline__ void mbar_expect_tx_only(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ uint32_t cvt_bf16x2(float hi, float lo) {
   uint32_t d;
@@ -129,7 +148,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   float* const s_b2 = s_g + 256;
   // the warp index is broadcast from lane 0 so that the compiler knows it is warp-uniform
   const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int cwg = warp >> 2, w = warp & 3, q = lane & 3;
+  const int w = warp & 3, q = lane & 3;
   // row -> (destination slot, neighbour slot): k is a power of two for every shipped configuration but 48
   const int kshift = (k & (k - 1)) == 0 ? __ffs(k) - 1 : -1;
   auto row_dst = [&](long long idx, int& j) -> unsigned {
@@ -143,23 +162,81 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   const long long n_rows = n_dst * k, split_rows = split_dst * k;      // both multiples of 128 by construction of the lists
   const long long n_tiles = (n_rows + kTile - 1) / kTile;
   const long long my_tiles = (n_tiles > blockIdx.x) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+  // P stage c: full[c] (producer -> consumer c, 32 producer lanes + the bytes of the copies), empty[c] (consumer c's 128 threads)
+  auto full_bar = [&](int c) { return sBar + 8u * (1 + c); };
+  auto empty_bar = [&](int c) { return sBar + 8u * (1 + kCons + c); };
 
   // ---- one-time setup: weight image and both class tables -> smem (TMA bulk copies), LayerNorm / bias vectors -> smem
   constexpr int kWAtom = NOUT * 128;            // one K-half of a weight piece: NOUT rows x 128 B
   constexpr int kWPiece = 2 * kWAtom;
   if (tid == 0) {
     mbar_init(sBar, 1);
+    for (int c = 0; c < kCons; ++c) { mbar_init(full_bar(c), 32); mbar_init(empty_bar(c), 128); }
     fence_barrier_init();
     mbar_expect_tx(sBar, 2u * kWPiece + 2u * kTabClassBytes);
     bulk_g2s(sW, w2_image, 2u * kWPiece, sBar);
     bulk_g2s(sT, tab_image, 2u * kTabClassBytes, sBar);
   }
   for (int i = tid; i < 128; i += kThreads) { s_g[i] = lp.g[i]; s_b[i] = lp.b[i]; s_b2[i] = lp.b2[i]; }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ================================================================= producer
+    setmaxnreg_dec<kProdRegs>();
+    // producer warp c fills stage c for consumer c.  A tile's metadata is gathered before the wait for the stage, so only the bulk
+    // copies remain between the consumer's hand-back and its next tile.
+    if (warp >= kCons) return;
+    const int c = warp;
+    const uint32_t st = sbase + oStage + (uint32_t)c * kStage;
+    for (long long it = c, use = 0; it < my_tiles; it += kCons, ++use) {
+      const long long tile = blockIdx.x + it * (long long)gridDim.x, row0 = tile * kTile;
+      int j0;
+      const unsigned a0 = row_dst(row0, j0);
+      const long long last = (row0 + kTile - 1 < n_rows ? row0 + kTile - 1 : n_rows - 1);
+      const int n_d = min(kDst, (int)(row_dst(last, j0) - a0) + 1);   // destinations with a staged P[dst] row
+      int s[2];
+      int4 meta[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long long idx = row0 + lane + 32 * h;
+        int jj = 0, ty = 3, slot = 0, node = -1;
+        float dist = 0.f;
+        s[h] = -1;
+        if (idx < n_rows) {
+          const unsigned a = row_dst(idx, jj);
+          slot = a - a0 < (unsigned)kDst ? (int)(a - a0) + 1 : 0;
+          node = row_nodes[a];
+          if (node >= 0) {
+            const size_t e = (size_t)node * k + jj;
+            s[h] = src[e]; ty = etype[e]; dist = dist_arr[e];
+          }
+        }
+        meta[h] = make_int4(node, s[h], __float_as_int(dist), ty | (slot << 8) | (jj << 16));
+      }
+      int dnode = -1;
+      if (lane < n_d) dnode = row_nodes[a0 + lane];
+      mbar_wait(empty_bar(c), (uint32_t)(use & 1) ^ 1u);              // the first use of a stage passes at once
+#pragma unroll
+      for (int h = 0; h < 2; ++h) *reinterpret_cast<int4*>(smem_raw + oStage + c * kStage + sMeta + 16 * (lane + 32 * h)) = meta[h];
+      if (lane == 0) mbar_expect_tx_only(full_bar(c), (uint32_t)(kTile + n_d) * 512u);
+      __syncwarp();
+      // absent slots read the all-zero row `zero_row` kept by the engine
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        bulk_g2s(st + sSrc + (uint32_t)(lane + 32 * h) * kSrcStride, P + (size_t)(s[h] >= 0 ? s[h] : zero_row) * TD_NPROJ + offB, 512u, full_bar(c));
+      if (lane < n_d) bulk_g2s(st + sDstRows + (uint32_t)lane * 512u, P + (size_t)(dnode >= 0 ? dnode : zero_row) * TD_NPROJ + offA, 512u, full_bar(c));
+      mbar_arrive(full_bar(c));
+    }
+    return;
+  }
+
+  // ================================================================= consumers
+  setmaxnreg_inc<kConsRegs>();
+  const int cwg = (warp >> 2) - 1;
   float mu[5];
 #pragma unroll
   for (int m = 0; m < 5; ++m) mu[m] = lp.mu[5 * q + m];
   const float coeff2 = coeff * 1.4426950408889634f;
-  __syncthreads();
   mbar_wait(sBar, 0);
 
   const int r_base = 16 * w + (lane >> 2);
@@ -168,43 +245,35 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   float* const xpart = xslot + ((w & 1) ? -256 : 256);
   const bool do_agg = NOUT == 128 && qnode == nullptr && agg.logits != nullptr;
   const bool key_sm = NOUT == 128 && qnode != nullptr && agg.key_softmax;
+  const unsigned char* const stage = smem_raw + oStage + cwg * kStage;
+  // MMA phase order: consumer 0 first, then strictly alternating.  Every consumer runs the same number of iterations (one without
+  // a tile only passes the order on); consumer 1's first hand-over and consumer 0's wait after the loop keep the counts equal, so
+  // no barrier is left half-arrived.
+  const int order_mine = kOrderBar + cwg, order_other = kOrderBar + (cwg ^ 1);
+  const long long n_iter = (my_tiles + kCons - 1) / kCons;
+  if (n_iter == 0) return;
+  if (cwg == 1) named_bar_arrive(order_other, 256);
   int set = 0;
 
-  for (long long it = cwg; it < my_tiles; it += kCons, set ^= 1) {
+  for (long long n = 0; n < n_iter; ++n, set ^= 1) {
+    const long long it = n * kCons + cwg;
+    if (it >= my_tiles) {
+      for (int phase = 0; phase < 2; ++phase) { named_bar_sync(order_mine, 256); named_bar_arrive(order_other, 256); }
+      continue;
+    }
     const long long tile = blockIdx.x + it * (long long)gridDim.x;
     const int cls = (tile * kTile >= split_rows) ? 1 : 0;
     // ---- metadata of this thread's two rows (s < 0: absent edge / padding destination / beyond the end)
     long long idx[2];
-    int node[2], s[2], ty[2], jj[2];
+    int node[2], s[2], ty[2], jj[2], dsl[2];
     float dist[2];
+    mbar_wait(full_bar(cwg), (uint32_t)(n & 1));
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       idx[h] = tile * kTile + r_base + 8 * h;
-      node[h] = -1; s[h] = -1; ty[h] = 3; jj[h] = 0; dist[h] = 0.f;
-      if (idx[h] < n_rows) {
-        const unsigned a = row_dst(idx[h], jj[h]);
-        node[h] = row_nodes[a];
-        if (node[h] >= 0) {
-          const size_t e = (size_t)node[h] * k + jj[h];
-          s[h] = src[e]; ty[h] = etype[e]; dist[h] = dist_arr[e];
-        }
-      }
-    }
-    // ---- P[src, offB ..] (absent slots read the all-zero row `zero_row` kept by the engine) + P[dst, offA ..], in fragment order
-    float x[64];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const bool valid = s[h] >= 0;
-      const float* ps = P + (size_t)(valid ? s[h] : zero_row) * TD_NPROJ + offB + 2 * q;
-      const float* pd = P + (size_t)(valid ? node[h] : zero_row) * TD_NPROJ + offA + 2 * q;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(ps + 8 * i));
-        float2 a = make_float2(0.f, 0.f);
-        if (valid) a = __ldg(reinterpret_cast<const float2*>(pd + 8 * i));
-        x[4 * i + 2 * h] = __fadd_rn(b.x, a.x);
-        x[4 * i + 2 * h + 1] = __fadd_rn(b.y, a.y);
-      }
+      const int4 m4 = *reinterpret_cast<const int4*>(stage + sMeta + 16 * (r_base + 8 * h));
+      node[h] = m4.x; s[h] = m4.y; dist[h] = __int_as_float(m4.z);
+      ty[h] = m4.w & 0xff; dsl[h] = ((m4.w >> 8) & 0xff) - 1; jj[h] = m4.w >> 16;
     }
     // ---- G in the A fragment: K-slot half 0 = edge from a protein atom (types 3 / 2), half 1 = from a ligand atom (types 1 / 0).
     //      Inside the row's half, this lane's slots (kk, register) carry m = 4 (kk % 2) + 2 (register / 2) + {0, 1}: gaussian 5 q + m
@@ -233,23 +302,38 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
           glo[kk][h + 2 * hk] = own ? lo : 0u;
         }
     }
-    // ---- Dpre = G . TabClass^T   (K = 64: four K=16 instructions per product term)
-    {
-      float d[64];
-      const uint32_t sTc = sT + (uint32_t)cls * kTabClassBytes;
-      wgmma_fence();
+    // ---- Dpre = G . TabClass^T   (K = 64: four K=16 instructions per product term), then x = (P[src] + P[dst]) + Dpre
+    float x[64];
+    const uint32_t sTc = sT + (uint32_t)cls * kTabClassBytes;
+    wgmma_fence();
+    named_bar_sync(order_mine, 256);
 #pragma unroll
-      for (int term = 0; term < 3; ++term) {
+    for (int term = 0; term < 3; ++term) {
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          wgmma_n128_rs(d, term == 2 ? glo[kk] : ghi[kk], gmma_desc_sw128(sTc + (term == 1 ? kTabClassBytes / 2 : 0) + kk * 32),
-                        (term | kk) ? 1u : 0u);     // a1b1, a1b2, a2b1
-      }
-      wgmma_commit();
-      wgmma_wait_all();
-#pragma unroll
-      for (int i = 0; i < 64; ++i) x[i] = __fadd_rn(x[i], d[i]);
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_n128_rs(x, term == 2 ? glo[kk] : ghi[kk], gmma_desc_sw128(sTc + (term == 1 ? kTabClassBytes / 2 : 0) + kk * 32),
+                      (term | kk) ? 1u : 0u);     // a1b1, a1b2, a2b1
     }
+    wgmma_commit();
+    named_bar_arrive(order_other, 256);
+    wgmma_wait_all();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const bool valid = s[h] >= 0;
+      const float* ps = reinterpret_cast<const float*>(stage + sSrc + (r_base + 8 * h) * kSrcStride) + 2 * q;
+      // P[dst]: the staged row, or (a destination beyond the first kDst of the tile) global memory
+      const float* pd = (dsl[h] >= 0 ? reinterpret_cast<const float*>(stage + sDstRows + dsl[h] * 512)
+                                     : P + (size_t)(valid ? node[h] : zero_row) * TD_NPROJ + offA) + 2 * q;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const float2 b = *reinterpret_cast<const float2*>(ps + 8 * i);
+        float2 a = make_float2(0.f, 0.f);
+        if (valid) a = *reinterpret_cast<const float2*>(pd + 8 * i);
+        x[4 * i + 2 * h] = __fadd_rn(__fadd_rn(b.x, a.x), x[4 * i + 2 * h]);
+        x[4 * i + 2 * h + 1] = __fadd_rn(__fadd_rn(b.y, a.y), x[4 * i + 2 * h + 1]);
+      }
+    }
+    mbar_arrive(empty_bar(cwg));                                  // P stage read: the producer may refill it
     // ---- LayerNorm over the 128 features of each row: 32 per lane, the 4 lanes of the quad combine by shuffles
     float rstd[2];
 #pragma unroll
@@ -289,6 +373,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
     // ---- D = hid . W2^T
     float o[NOUT / 2];
     wgmma_fence();
+    named_bar_sync(order_mine, 256);
 #pragma unroll
     for (int term = 0; term < 3; ++term) {
 #pragma unroll
@@ -299,6 +384,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       }
     }
     wgmma_commit();
+    named_bar_arrive(order_other, 256);
     wgmma_wait_all();
 
     // ================================================================= epilogue on the D fragment
@@ -399,9 +485,8 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
         for (int h = 0; h < 2; ++h) {
           valid_e[h] = false; ew[h] = 0.f;
           if (owrite[h]) {
-            const size_t e = (size_t)node[h] * k + jj[h];
-            valid_e[h] = src[e] >= 0;
-            ew[h] = agg.e_w[e];
+            valid_e[h] = s[h] >= 0;
+            ew[h] = agg.e_w[(size_t)node[h] * k + jj[h]];
           }
         }
         float mx[4], sm[4];
@@ -446,6 +531,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       }
     }
   }
+  if (cwg == 0) named_bar_sync(order_mine, 256);                 // matches consumer 1's last hand-over
 }
 
 // n_dst destinations (device counts {n_dst, split_dst} in d_counts override the host values); see the kernel comment for the row model
