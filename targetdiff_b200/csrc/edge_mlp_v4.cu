@@ -6,6 +6,11 @@
 //   hid     = relu(LN(pre) * ln_g + ln_b)
 //   out[e]  = hid . W2^T + b2
 //
+//   Packer contract (engine.cu, pack_edge_mlp with sign_in_w1): every term of pre comes from a first Linear whose rows are centred over
+//   the 128 features and multiplied by the sign of the LayerNorm gain, and the gain's magnitude is folded into W2 / b2.  So pre arrives
+//   as s * (pre - mean(pre)) and the LayerNorm reduces to  hid = relu(pre * rsqrt(sum(pre^2) / 128 + eps) + ln_b):  no mean pass and
+//   no gain (ln_g = 1 is not read).  The mean left by rounding is ~1e-6 of the row's scale; its effect on the variance is its square.
+//
 //   * rows are visited through a CLASS-SORTED destination list (protein destinations, padded to a tile multiple, then ligand
 //     destinations): a tile holds destinations of one class, hence at most two edge types -- protein destination: P->P (3) or
 //     L->P (1); ligand destination: P->L (2) or L->L (0).  The gaussian/type block of BOTH is one small MMA
@@ -19,10 +24,10 @@
 // CTA = one producer warpgroup + kCons consumer warpgroups, one CTA per SM, persistent over tiles of 64 edge rows (one wgmma M).
 // The producer (one warp per consumer; `setmaxnreg` leaves it 40 registers and gives the consumers 232) stages each tile in shared
 // memory ahead of its consumer: the rows' metadata and the P[src] / P[dst] rows as 512-byte bulk copies.  Consumer c takes the CTA's tiles
-// c, c + kCons, ... and owns P stage c, which it hands back right after reading it (before the LayerNorm).  The two consumers'
+// c, c + kCons, ... and owns P stage c, which it hands back right after reading it (before its pre-MMA).  The two consumers'
 // tensor-core phases (pre-MMA, main MMA) run in a fixed alternating order (two named barriers): one consumer's MMAs are issued
 // whole while the other does its LayerNorm, split and epilogue, so the two never interleave on the tensor cores.
-// Shared memory: W2 pieces 64 KB | both class tables 64 KB | LayerNorm affine + b2 1.5 KB | exchange slots 4 KB per consumer |
+// Shared memory: W2 pieces 64 KB | both class tables 64 KB | ln_b + b2 1 KB | exchange slots 4 KB per consumer |
 // 2 P stages of 39 KB (64 P[src] rows with a 544-byte stride, which makes the fragment-order reads free of bank conflicts,
 // kDst P[dst] rows, 64 metadata records) | mbarriers.
 #include <stdio.h>
@@ -45,7 +50,7 @@ constexpr int kProdRegs = 40, kConsRegs = 232;  // setmaxnreg: 128 * 40 + 2 * 12
 constexpr int kSrcStride = 512 + 32, kDst = 8;
 constexpr int sSrc = 0, sDstRows = sSrc + kTile * kSrcStride, sMeta = sDstRows + kDst * 512, kStage = sMeta + kTile * 16;
 // shared-memory map (bytes from the 1024-aligned base)
-constexpr int oW = 0, oT = oW + 4 * 128 * 128, oPar = oT + 2 * kTabClassBytes, oX = oPar + 3 * 128 * 4, oStage = oX + kCons * 4 * 2 * 128 * 4,
+constexpr int oW = 0, oT = oW + 4 * 128 * 128, oPar = oT + 2 * kTabClassBytes, oX = oPar + 2 * 128 * 4, oStage = oX + kCons * 4 * 2 * 128 * 4,
               oBar = oStage + kCons * kStage, kSmem = oBar + 8 * (1 + 2 * kCons);   // barriers: weights, full[kCons], empty[kCons]
 static_assert(oStage % 128 == 0 && kStage % 128 == 0 && kSmem <= 227 * 1024, "shared-memory map");
 constexpr int kOrderBar = 5;               // named barriers kOrderBar + c: consumer c may issue its next MMA phase (1-4: warp pairs)
@@ -88,8 +93,8 @@ __device__ __forceinline__ void stg128(float* p, float a, float b, float c, floa
   asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
-// LayerNorm affine parameters, the output bias and the gaussian centres travel as a kernel argument (copied to shared memory)
-struct LnParams { float g[128]; float b[128]; float b2[128]; float mu[20]; };
+// LayerNorm bias, the output bias and the gaussian centres travel as a kernel argument (copied to shared memory)
+struct LnParams { float b[128]; float b2[128]; float mu[20]; };
 // Fused attention in the epilogues (k == 32: rows 0-31 and 32-63 of a tile are the edges of one destination each, held by warps
 // {0, 1} and {2, 3} of the warpgroup), reference models/uni_transformer.py:73-83:  key launch writes softmax_e(q.k/sqrt 8) * e_w,
 // value launch does h[dst] += sum_e w * v.
@@ -143,9 +148,8 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t sbase = smem_u32(smem_raw);
   const uint32_t sW = sbase + oW, sT = sbase + oT, sBar = sbase + oBar;
-  float* const s_g = reinterpret_cast<float*>(smem_raw + oPar);       // ln_g | ln_b | b2
-  float* const s_b = s_g + 128;
-  float* const s_b2 = s_g + 256;
+  float* const s_b = reinterpret_cast<float*>(smem_raw + oPar);       // ln_b | b2
+  float* const s_b2 = s_b + 128;
   // the warp index is broadcast from lane 0 so that the compiler knows it is warp-uniform
   const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   const int w = warp & 3, q = lane & 3;
@@ -166,7 +170,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   auto full_bar = [&](int c) { return sBar + 8u * (1 + c); };
   auto empty_bar = [&](int c) { return sBar + 8u * (1 + kCons + c); };
 
-  // ---- one-time setup: weight image and both class tables -> smem (TMA bulk copies), LayerNorm / bias vectors -> smem
+  // ---- one-time setup: weight image and both class tables -> smem (TMA bulk copies), bias vectors -> smem
   constexpr int kWAtom = NOUT * 128;            // one K-half of a weight piece: NOUT rows x 128 B
   constexpr int kWPiece = 2 * kWAtom;
   if (tid == 0) {
@@ -177,7 +181,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
     bulk_g2s(sW, w2_image, 2u * kWPiece, sBar);
     bulk_g2s(sT, tab_image, 2u * kTabClassBytes, sBar);
   }
-  for (int i = tid; i < 128; i += kThreads) { s_g[i] = lp.g[i]; s_b[i] = lp.b[i]; s_b2[i] = lp.b2[i]; }
+  for (int i = tid; i < 128; i += kThreads) { s_b[i] = lp.b[i]; s_b2[i] = lp.b2[i]; }
   __syncthreads();
 
   if (warp < 4) {
@@ -302,21 +306,9 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
           glo[kk][h + 2 * hk] = own ? lo : 0u;
         }
     }
-    // ---- Dpre = G . TabClass^T   (K = 64: four K=16 instructions per product term), then x = (P[src] + P[dst]) + Dpre
+    // ---- x = P[src] + P[dst] from the stage, which then goes back to the producer; the pre-MMA adds Dpre = G . TabClass^T to it
+    //      (K = 64: four K=16 instructions per product term), so the tensor core does that add and the stage is free before the MMA
     float x[64];
-    const uint32_t sTc = sT + (uint32_t)cls * kTabClassBytes;
-    wgmma_fence();
-    named_bar_sync(order_mine, 256);
-#pragma unroll
-    for (int term = 0; term < 3; ++term) {
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk)
-        wgmma_n128_rs(x, term == 2 ? glo[kk] : ghi[kk], gmma_desc_sw128(sTc + (term == 1 ? kTabClassBytes / 2 : 0) + kk * 32),
-                      (term | kk) ? 1u : 0u);     // a1b1, a1b2, a2b1
-    }
-    wgmma_commit();
-    named_bar_arrive(order_other, 256);
-    wgmma_wait_all();
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const bool valid = s[h] >= 0;
@@ -329,36 +321,41 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
         const float2 b = *reinterpret_cast<const float2*>(ps + 8 * i);
         float2 a = make_float2(0.f, 0.f);
         if (valid) a = *reinterpret_cast<const float2*>(pd + 8 * i);
-        x[4 * i + 2 * h] = __fadd_rn(__fadd_rn(b.x, a.x), x[4 * i + 2 * h]);
-        x[4 * i + 2 * h + 1] = __fadd_rn(__fadd_rn(b.y, a.y), x[4 * i + 2 * h + 1]);
+        x[4 * i + 2 * h] = __fadd_rn(b.x, a.x);
+        x[4 * i + 2 * h + 1] = __fadd_rn(b.y, a.y);
       }
     }
     mbar_arrive(empty_bar(cwg));                                  // P stage read: the producer may refill it
-    // ---- LayerNorm over the 128 features of each row: 32 per lane, the 4 lanes of the quad combine by shuffles
+    const uint32_t sTc = sT + (uint32_t)cls * kTabClassBytes;
+    wgmma_fence();
+    named_bar_sync(order_mine, 256);
+#pragma unroll
+    for (int term = 0; term < 3; ++term) {
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_n128_rs(x, term == 2 ? glo[kk] : ghi[kk], gmma_desc_sw128(sTc + (term == 1 ? kTabClassBytes / 2 : 0) + kk * 32),
+                      1u);                        // a1b1, a1b2, a2b1
+    }
+    wgmma_commit();
+    named_bar_arrive(order_other, 256);
+    wgmma_wait_all();
+    // ---- LayerNorm over the 128 features of each row (centred by the packer: the variance is the mean square): 32 per lane, the 4
+    //      lanes of the quad combine by shuffles
     float rstd[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      float sa = 0.f, sb = 0.f;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) { sa = __fadd_rn(sa, x[4 * i + 2 * h]); sb = __fadd_rn(sb, x[4 * i + 2 * h + 1]); }
-      float sum = sa + sb;
-      sum += __shfl_xor_sync(0xffffffffu, sum, 1);
-      sum += __shfl_xor_sync(0xffffffffu, sum, 2);
-      const float mean = sum * (1.0f / 128.0f);
       float qa = 0.f, qb = 0.f;
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
-        float& x0 = x[4 * i + 2 * h];
-        float& x1 = x[4 * i + 2 * h + 1];
-        x0 = __fsub_rn(x0, mean); x1 = __fsub_rn(x1, mean);
-        qa = __fmaf_rn(x0, x0, qa); qb = __fmaf_rn(x1, x1, qb);
+        qa = __fmaf_rn(x[4 * i + 2 * h], x[4 * i + 2 * h], qa);
+        qb = __fmaf_rn(x[4 * i + 2 * h + 1], x[4 * i + 2 * h + 1], qb);
       }
       float var = qa + qb;
       var += __shfl_xor_sync(0xffffffffu, var, 1);
       var += __shfl_xor_sync(0xffffffffu, var, 2);
       rstd[h] = rsqrtf(var * (1.0f / 128.0f) + 1e-5f);
     }
-    // ---- affine + ReLU, bf16 split: the accumulator columns 16 kk .. 16 kk + 15 are the A fragment of K step kk.
+    // ---- normalise + bias + ReLU (unit gain), bf16 split: the accumulator columns 16 kk .. 16 kk + 15 are the A fragment of K step kk.
     //      Absent rows carry x = P[zero_row] + Dpre(0): their (finite) outputs are never consumed.
     uint32_t ahi[8][4], alo[8][4];
 #pragma unroll
@@ -366,8 +363,8 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
 #pragma unroll
       for (int r = 0; r < 4; ++r) {
         const int h = r & 1, col = 16 * kk + 8 * (r >> 1) + 2 * q, e = 8 * kk + 2 * r;
-        const float2 g = *reinterpret_cast<const float2*>(s_g + col), b = *reinterpret_cast<const float2*>(s_b + col);
-        const float y0 = __fmaf_rn(x[e], __fmul_rn(rstd[h], g.x), b.x), y1 = __fmaf_rn(x[e + 1], __fmul_rn(rstd[h], g.y), b.y);
+        const float2 b = *reinterpret_cast<const float2*>(s_b + col);
+        const float y0 = __fmaf_rn(x[e], rstd[h], b.x), y1 = __fmaf_rn(x[e + 1], rstd[h], b.y);
         split2(fmaxf(y0, 0.f), fmaxf(y1, 0.f), ahi[kk][r], alo[kk][r]);
       }
     // ---- D = hid . W2^T
@@ -537,11 +534,10 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
 // n_dst destinations (device counts {n_dst, split_dst} in d_counts override the host values); see the kernel comment for the row model
 void td_launch_edge_mlp_v4(const float* P, int zero_row, const int* src, const unsigned char* etype, const float* dist, const int* row_nodes, long long n_dst,
                            long long split_dst, const int* d_counts, int k, const TdMlp& m, const float* h_offsets, float coeff,
-                           const float* h_ln_g, const float* h_ln_b, const float* h_b2, const float* qnode, float* out, int out_by_slot,
+                           const float* h_ln_b, const float* h_b2, const float* qnode, float* out, int out_by_slot,
                            const float* agg_logits, const float* agg_e_w, float* agg_h, int key_softmax, int sm_count, cudaStream_t st) {
   if (n_dst == 0) return;
   LnParams lp;
-  memcpy(lp.g, h_ln_g, sizeof(lp.g));
   memcpy(lp.b, h_ln_b, sizeof(lp.b));
   memset(lp.b2, 0, sizeof(lp.b2));
   memcpy(lp.b2, h_b2, sizeof(float) * (size_t)m.nout);

@@ -15,6 +15,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <list>
 #include <map>
 #include <string>
 #include <vector>
@@ -127,6 +128,7 @@ struct Packer {
   std::vector<float> host;
   std::vector<unsigned char> img;
   std::string missing;
+  std::list<std::vector<float>> keep;   // reparameterised weights that later packing steps still read (stable addresses)
   const float* get(const std::string& name, int64_t numel) {
     auto it = byname.find(name);
     if (it == byname.end() || it->second->numel != numel || it->second->data == nullptr) {
@@ -194,16 +196,51 @@ void pack_tabcls_image(const float* tab /*[4][21][128]*/, std::vector<unsigned c
       }
 }
 
-// edge MLP: first Linear [128, 4 + 80 + 128 + 128] split, LayerNorm affine, second Linear transposed
-bool pack_edge_mlp(Packer& pk, const std::string& p, int nout, MlpOff& o, const float** w1_out) {
+// Reparameterisation of an edge MLP  hid = relu(LN(pre) * g + b), out = hid . W2^T + b2,  pre = W1 . input + b1  (exact in real
+// arithmetic), applied before anything is derived from its weights.  For first-layer output feature f, s_f = sign(g_f) (+1 for g_f = 0):
+//  * centre W1 / b1 over the 128 output features: W1[f,:] -= mean_f' W1[f',:], b1[f] -= mean(b1).  Every term of the pre-activation
+//    (type column, gaussians, h[dst], h[src]) comes through W1 / b1, so pre arrives with zero mean; LayerNorm is shift-invariant;
+//  * fold the gain's magnitude into the second Linear: relu(g x + b) = |g| relu(s x + b / |g|), so ln_b = b / |g| and W2[:,f] *= |g|.
+//    A feature with g_f = 0, or b_f / |g_f| not finite, is the constant relu(b_f): relu(b_f) W2[:,f] moves into b2, the column is 0;
+//  * s goes into W1's row f (sign_in_w1, ln_g = 1) for edge_mlp_v4.cu, whose LayerNorm is then x * rsqrt(mean(x^2) + eps) + ln_b
+//    with no mean and no gain; otherwise ln_g = s: the older kernels subtract the row mean, which flipping some rows would change.
+// The class tables, the node-projection blocks (wn_t and its images) and the fp32 tables all inherit the transformed W1 (*w1_out).
+// First Linear [128, 4 + 80 + 128 + 128] split, LayerNorm affine, second Linear transposed.
+bool pack_edge_mlp(Packer& pk, const std::string& p, int nout, bool sign_in_w1, MlpOff& o, const float** w1_out) {
   const int KV = 4 + 4 * TD_NG + 2 * TD_H;
-  const float* w1 = pk.get(p + ".net.0.weight", (int64_t)TD_H * KV);
-  const float* b1 = pk.get(p + ".net.0.bias", TD_H);
-  const float* g = pk.get(p + ".net.1.weight", TD_H);
-  const float* b = pk.get(p + ".net.1.bias", TD_H);
-  const float* w2 = pk.get(p + ".net.3.weight", (int64_t)nout * TD_H);
-  const float* b2 = pk.get(p + ".net.3.bias", nout);
-  if (!w1 || !b1 || !g || !b || !w2 || !b2) return false;
+  const float* w1_in = pk.get(p + ".net.0.weight", (int64_t)TD_H * KV);
+  const float* b1_in = pk.get(p + ".net.0.bias", TD_H);
+  const float* g_in = pk.get(p + ".net.1.weight", TD_H);
+  const float* b_in = pk.get(p + ".net.1.bias", TD_H);
+  const float* w2_in = pk.get(p + ".net.3.weight", (int64_t)nout * TD_H);
+  const float* b2_in = pk.get(p + ".net.3.bias", nout);
+  if (!w1_in || !b1_in || !g_in || !b_in || !w2_in || !b2_in) return false;
+  std::vector<float>& w1v = pk.keep.emplace_back((size_t)TD_H * KV);
+  std::vector<float> b1v(TD_H), gv(TD_H), bv(TD_H), w2v((size_t)nout * TD_H), b2v(nout);
+  {
+    std::vector<double> mw(KV, 0.0), b2acc(b2_in, b2_in + nout);
+    double mb = 0.0;
+    for (int f = 0; f < TD_H; ++f) {
+      for (int j = 0; j < KV; ++j) mw[j] += w1_in[(size_t)f * KV + j];
+      mb += b1_in[f];
+    }
+    for (int f = 0; f < TD_H; ++f) {
+      const double s = g_in[f] < 0.0f ? -1.0 : 1.0, ag = fabs((double)g_in[f]), s1 = sign_in_w1 ? s : 1.0;
+      for (int j = 0; j < KV; ++j) w1v[(size_t)f * KV + j] = (float)(s1 * (w1_in[(size_t)f * KV + j] - mw[j] / TD_H));
+      b1v[f] = (float)(s1 * (b1_in[f] - mb / TD_H));
+      gv[f] = (float)(s / s1);
+      const float bf = (float)(b_in[f] / ag);
+      const bool constant = g_in[f] == 0.0f || !isfinite(bf);
+      bv[f] = constant ? 0.0f : bf;
+      for (int n = 0; n < nout; ++n) {
+        const double w = w2_in[(size_t)n * TD_H + f];
+        w2v[(size_t)n * TD_H + f] = constant ? 0.0f : (float)(ag * w);
+        if (constant && b_in[f] > 0.0f) b2acc[n] += (double)b_in[f] * w;
+      }
+    }
+    for (int n = 0; n < nout; ++n) b2v[n] = (float)b2acc[n];
+  }
+  const float *w1 = w1v.data(), *b1 = b1v.data(), *g = gv.data(), *b = bv.data(), *w2 = w2v.data(), *b2 = b2v.data();
   o.nout = nout;
   o.tab = pk.alloc(4 * TD_TAB * TD_H);
   for (int t = 0; t < 4; ++t) {
@@ -275,11 +312,11 @@ bool pack_sublayer_options(Packer& pk, const std::string& p, int ew_dim, bool ou
   return true;
 }
 
-bool pack_sublayer(Packer& pk, const std::string& p, const char* kn, const char* vn, const char* qn, int nout_v, SubOff& so) {
+bool pack_sublayer(Packer& pk, const std::string& p, const char* kn, const char* vn, const char* qn, int nout_v, bool sign_in_w1, SubOff& so) {
   const int KV = 4 + 4 * TD_NG + 2 * TD_H;
   const float *w1k = nullptr, *w1v = nullptr;
-  if (!pack_edge_mlp(pk, p + "." + kn, TD_H, so.k, &w1k)) return false;
-  if (!pack_edge_mlp(pk, p + "." + vn, nout_v, so.v, &w1v)) return false;
+  if (!pack_edge_mlp(pk, p + "." + kn, TD_H, sign_in_w1, so.k, &w1k)) return false;
+  if (!pack_edge_mlp(pk, p + "." + vn, nout_v, sign_in_w1, so.v, &w1v)) return false;
   const std::string qp = p + "." + qn;
   const float* w1q = pk.get(qp + ".net.0.weight", (int64_t)TD_H * TD_H);
   const float* b1q = pk.get(qp + ".net.0.bias", TD_H);
@@ -369,6 +406,15 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
   tdiff_engine* e = new tdiff_engine();
   e->cfg = *cfg; e->device = device; e->sm_count = prop.multiProcessorCount; e->K = e->KQ = cfg->knn; e->hybrid = cfg->cutoff_mode;
   e->num_blocks = cfg->num_blocks > 1 ? cfg->num_blocks : 1; e->ew_mode = cfg->ew_net_type; e->out_fc = cfg->x2h_out_fc; e->time_emb = cfg->time_emb;
+  // the edge-MLP mode decides where the packer puts the LayerNorm gain's sign (pack_edge_mlp)
+  if (const char* mode = getenv("TDIFF_EDGE_MLP")) {
+    if (!strcmp(mode, "simt")) e->mlp_mode = 0;
+    else if (!strcmp(mode, "tc3")) e->mlp_mode = 2;
+    else if (!strcmp(mode, "tc3v2")) { e->mlp_mode = 2; e->mlp_v4 = false; }
+    else if (!strcmp(mode, "tc6")) e->mlp_mode = 3;
+    else { delete e; return set_err(TDIFF_EINVAL, "TDIFF_EDGE_MLP=%s (simt|tc3|tc3v2|tc6)", mode); }
+  }
+  const bool v4 = e->mlp_mode == 2 && e->mlp_v4;
 
   Packer pk;
   for (int i = 0; i < n_entries; ++i)
@@ -437,8 +483,8 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
   std::vector<float> coeffs(L, -0.5f);
   for (int l = 0; l < L; ++l) {
     const std::string p = "refine_net.base_block." + std::to_string(l);
-    if (!pack_sublayer(pk, p + ".x2h_layers.0", "hk_func", "hv_func", "hq_func", TD_H, sx[l])) break;
-    if (!pack_sublayer(pk, p + ".h2x_layers.0", "xk_func", "xv_func", "xq_func", TD_HEADS, sh[l])) break;
+    if (!pack_sublayer(pk, p + ".x2h_layers.0", "hk_func", "hv_func", "hq_func", TD_H, v4, sx[l])) break;
+    if (!pack_sublayer(pk, p + ".h2x_layers.0", "xk_func", "xv_func", "xq_func", TD_HEADS, v4, sh[l])) break;
     if (!pack_sublayer_options(pk, p + ".x2h_layers.0", cfg->ew_net_type == 1 ? 4 * TD_NG : cfg->ew_net_type == 2 ? TD_H : 0, cfg->x2h_out_fc != 0, sx[l])) break;
     if (!pack_sublayer_options(pk, p + ".h2x_layers.0", cfg->ew_net_type == 1 ? 4 * TD_NG : 0, false, sh[l])) break;
     const float* off = pk.get(p + ".distance_expansion.offset", TD_NG);
@@ -463,13 +509,6 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
         cudaMemcpy(e->img_arena, pk.img.data(), pk.img.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
       cudaFree(e->arena); delete e; return set_err(TDIFF_ECUDA, "weight image upload failed");
     }
-  }
-  if (const char* mode = getenv("TDIFF_EDGE_MLP")) {
-    if (!strcmp(mode, "simt")) e->mlp_mode = 0;
-    else if (!strcmp(mode, "tc3")) e->mlp_mode = 2;
-    else if (!strcmp(mode, "tc3v2")) { e->mlp_mode = 2; e->mlp_v4 = false; }
-    else if (!strcmp(mode, "tc6")) e->mlp_mode = 3;
-    else { cudaFree(e->arena); cudaFree(e->img_arena); delete e; return set_err(TDIFF_EINVAL, "TDIFF_EDGE_MLP=%s (simt|tc3|tc3v2|tc6)", mode); }
   }
   if ((cfg->ew_net_type != 0 || cfg->x2h_out_fc || cfg->cutoff_mode != 0) && !(e->mlp_mode == 2 && e->mlp_v4)) {
     cudaFree(e->arena); cudaFree(e->img_arena); delete e;
@@ -742,7 +781,7 @@ void edge_mlp(tdiff_engine* e, const float* P, const float4* xm, const int* src,
     // plain (unfused) x2h outputs are consumed by slot index (aggregate_h_logits_kernel); everything else by row index
     const int by_slot = (list != ROWS_LIGAND && !key_softmax && agg_logits == nullptr) ? 1 : 0;
     td_launch_edge_mlp_v4(P, e->N, src, etype, e->dist.as<float>(), rows, n_dst, split, counts, K, m,
-                          e->host_arena.data() + (offsets - e->arena), coeff, e->host_arena.data() + (m.ln_g - e->arena), e->host_arena.data() + (m.ln_b - e->arena),
+                          e->host_arena.data() + (offsets - e->arena), coeff, e->host_arena.data() + (m.ln_b - e->arena),
                           e->host_arena.data() + (m.b2 - e->arena), qnode, out, by_slot, agg_logits, e_w, agg_h, key_softmax,
                           e->sm_count, st);
     return;

@@ -20,6 +20,8 @@
 // One 2-layer edge/node MLP after the exact first-layer split (SURVEY.md Appendix B):
 //   pre = P[dst, offA:] + P[src, offB:] + tab[type][20] + sum_j g_j * tab[type][j]      (edge MLPs)
 //   hid = relu(LN(pre) * ln_g + ln_b);  out = hid . w2t + b2
+// Edge MLPs are packed reparameterised (engine.cu, pack_edge_mlp): pre arrives centred, ln_g = +-1 (1 for the v4 kernel, whose pre also
+// carries the gain's sign), and the gain's magnitude is folded into w2t / w2_img.
 struct TdMlp {
   const float* tab;    // [4][TD_TAB][128] (edge MLPs only)
   const float* ln_g;   // [128]
@@ -172,7 +174,7 @@ void td_launch_edge_mlp_tc(const float* P, const float4* xm, const int* src, con
                            float* out, int sm_count, cudaStream_t st);
 void td_launch_edge_mlp_v4(const float* P, int zero_row, const int* src, const unsigned char* etype, const float* dist, const int* row_nodes, long long n_dst,
                            long long split_dst, const int* d_counts, int k, const TdMlp& m, const float* h_offsets, float coeff,
-                           const float* h_ln_g, const float* h_ln_b, const float* h_b2, const float* qnode, float* out, int out_by_slot,
+                           const float* h_ln_b, const float* h_b2, const float* qnode, float* out, int out_by_slot,
                            const float* agg_logits, const float* agg_e_w, float* agg_h, int key_softmax, int sm_count, cudaStream_t st);
 void td_launch_rows_tc(int mode, const float* in, int ldi, int in_off, long long n_rows, TdMlp m, const unsigned char* w_image, int pieces, float* out,
                        int ldo, int nblocks, const int* row_list, const int* d_n_rows, int sm_count, cudaStream_t st);
