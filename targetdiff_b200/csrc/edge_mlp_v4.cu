@@ -45,7 +45,7 @@ constexpr int kTile = 64;                  // rows per tile
 constexpr int kTabClassBytes = 2 * 128 * 128;   // one class table: 2 bf16 pieces of [128 x 64]
 constexpr int kProdRegs = 40, kConsRegs = 232;  // setmaxnreg: 128 * 40 + 2 * 128 * 232 = 384 * 168 (the launch's allocation)
 // P stage: P[src] rows (stride padded by 32 B: the 8 rows one fragment load touches fall in distinct banks), the tile's first kDst
-// destinations' P[dst] rows (k >= 10 never needs more; rows of further destinations are read from global memory), and per row
+// destinations' P[dst] rows (k >= 8 never needs more; rows of further destinations, k <= 7, are read from global memory), and per row
 // the metadata record {node, src, dist, type | (dst slot + 1) << 8 | neighbour slot << 16}
 constexpr int kSrcStride = 512 + 32, kDst = 8;
 constexpr int sSrc = 0, sDstRows = sSrc + kTile * kSrcStride, sMeta = sDstRows + kDst * 512, kStage = sMeta + kTile * 16;

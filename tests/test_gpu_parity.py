@@ -222,9 +222,11 @@ def test_chain_graph_replay_equals_eager(monkeypatch):
     args = (b['protein_pos'], b['protein_v'], b['batch_protein'], b['init_ligand_pos'], b['init_ligand_v'], b['batch_ligand'])
     r1 = model.sample_diffusion(*args, num_steps=S, center_pos_mode='protein', noise_tape=(pn, vu))
     monkeypatch.setenv('TDIFF_NO_GRAPH', '1')
+    model, _ = _model(5)                  # the switch is read when the engine is created: a fresh model, a fresh engine
     r2 = model.sample_diffusion(*args, num_steps=S, center_pos_mode='protein', noise_tape=(pn, vu))
     assert torch.equal(r1['pos'], r2['pos']) and torch.equal(r1['v'], r2['v'])
     assert torch.equal(torch.stack(r1['vt_traj']), torch.stack(r2['vt_traj']))
+    assert torch.equal(torch.stack(r1['pos_traj']), torch.stack(r2['pos_traj']))
 
 
 def test_chain_philox_reproducible_and_sane():
