@@ -29,7 +29,18 @@
 // whole while the other does its LayerNorm, split and epilogue, so the two never interleave on the tensor cores.
 // Shared memory: W2 pieces 64 KB | both class tables 64 KB | ln_b + b2 1 KB | exchange slots 4 KB per consumer |
 // 2 P stages of 39 KB (64 P[src] rows with a 544-byte stride, which makes the fragment-order reads free of bank conflicts,
-// kDst P[dst] rows, 64 metadata records) | mbarriers.
+// kDst P[dst] rows, 64 metadata records) | mbarriers.  215 KB.
+//
+// Folded key launch (FOLD, k = 32 or 64: a tile holds at most 2 destinations).  The key epilogue only needs
+//   logit[e, hd] = 1/sqrt(8) sum_d q[dst, 8 hd + d] (hid_e . W2^T + b2)[8 hd + d] = hid_e . M_dst[hd, :] + c_dst[hd],
+//   M_dst[hd, f] = 1/sqrt(8) sum_d q[dst, 8 hd + d] W2[8 hd + d, f],   c_dst[hd] = 1/sqrt(8) sum_d q[dst, 8 hd + d] b2[8 hd + d],
+// so the main MMA runs at N = 32 (16 heads x 2 destination slots) instead of 128.  The producer also stages the tile's q[dst] rows (in
+// P[dst] slots 2 and 3, unused for k >= 32); each consumer reads them before handing the stage back, builds M (fp32 W2 from shared
+// memory, CUDA cores, bf16-split) for its tile while its own pre-MMA runs, and preloads the accumulator with c_dst.  M row
+// n = 8 i + 2 q + c is head 4 q + 2 (i / 2) + c of destination slot i % 2, so lane q of a row's quad holds that row's heads
+// 4 q .. 4 q + 3 and the softmax / output need no exchange inside the quad.  One launch per destination class keeps one table resident.
+// Shared memory: W2 fp32 64 KB | the class table 32 KB | ln_b + b2 1 KB | exchange slots 8 KB | M images 16 KB per consumer |
+// c_dst 128 B per consumer | 2 P stages of 39 KB | mbarriers.  215 KB.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -49,11 +60,19 @@ constexpr int kProdRegs = 40, kConsRegs = 232;  // setmaxnreg: 128 * 40 + 2 * 12
 // the metadata record {node, src, dist, type | (dst slot + 1) << 8 | neighbour slot << 16}
 constexpr int kSrcStride = 512 + 32, kDst = 8;
 constexpr int sSrc = 0, sDstRows = sSrc + kTile * kSrcStride, sMeta = sDstRows + kDst * 512, kStage = sMeta + kTile * 16;
-// shared-memory map (bytes from the 1024-aligned base)
-constexpr int oW = 0, oT = oW + 4 * 128 * 128, oPar = oT + 2 * kTabClassBytes, oX = oPar + 2 * 128 * 4, oStage = oX + kCons * 4 * 2 * 128 * 4,
-              oBar = oStage + kCons * kStage, kSmem = oBar + 8 * (1 + 2 * kCons);   // barriers: weights, full[kCons], empty[kCons]
-static_assert(oStage % 128 == 0 && kStage % 128 == 0 && kSmem <= 227 * 1024, "shared-memory map");
+// folded key launch: per consumer the B image of M, 2 bf16 pieces of [32 rows x 128 K] (K halves of 32 x 128 B), and the 2 x 16 c_dst
+constexpr int kMAtom = 32 * 128, kMPiece = 2 * kMAtom, kMImg = 2 * kMPiece;
+// shared-memory map (bytes from the 1024-aligned base).  FOLD: W2 in fp32 instead of its bf16 image (both 64 KB), only the launch's
+// class table, plus the M images and c_dst.
+template <bool FOLD>
+struct Map {
+  static constexpr int W = 0, T = W + 4 * 128 * 128, Par = T + (FOLD ? 1 : 2) * kTabClassBytes, X = Par + 2 * 128 * 4,
+                       M = X + kCons * 4 * 2 * 128 * 4, C = M + (FOLD ? kCons * kMImg : 0), Stage = C + (FOLD ? kCons * 32 * 4 : 0),
+                       Bar = Stage + kCons * kStage, Smem = Bar + 8 * (1 + 2 * kCons);   // barriers: weights, full[kCons], empty[kCons]
+  static_assert(M % 1024 == 0 && Stage % 128 == 0 && kStage % 128 == 0 && Smem <= 227 * 1024, "shared-memory map");
+};
 constexpr int kOrderBar = 5;               // named barriers kOrderBar + c: consumer c may issue its next MMA phase (1-4: warp pairs)
+constexpr int kFoldBar = 7;                // named barriers kFoldBar + c: consumer c's M image is written
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -139,16 +158,21 @@ using namespace v4;
 //
 // Fragment ownership (thread t of warpgroup c, w = (t / 32) % 4, l = t % 32, q = l % 4): rows 16 w + l / 4 + 8 h (h = 0, 1), columns
 // 8 i + 2 q + {0, 1} (i < NOUT / 8) -- accumulator element d[4 i + 2 h + c] (hopper_mma.cuh).
-template <int NOUT>
+// FOLD (key MLPs, k = 32 or 64): the folded key path of the header; `w2_image` is then W2^T in fp32 ([128 f][128 out]) and the launch
+// covers the tiles of destination class `fold_cls` only (0: rows below split, 1: the rest).
+template <int NOUT, bool FOLD>
 __global__ void __launch_bounds__(kThreads, 1)
 edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restrict__ src, const unsigned char* __restrict__ etype,
                    const float* __restrict__ dist_arr, const int* __restrict__ row_nodes, long long n_dst, long long split_dst,
                    const int* __restrict__ d_counts, int k, int offA, int offB, const unsigned char* __restrict__ w2_image,
-                   const unsigned char* __restrict__ tab_image, float coeff, const float* __restrict__ qnode, float* __restrict__ out, int out_by_slot, AggArgs agg, const __grid_constant__ LnParams lp) {
+                   const unsigned char* __restrict__ tab_image, float coeff, const float* __restrict__ qnode, float* __restrict__ out, int out_by_slot, AggArgs agg,
+                   int fold_cls, const __grid_constant__ LnParams lp) {
+  static_assert(!FOLD || NOUT == 128, "the fold applies to the key MLPs");
+  using L = Map<FOLD>;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t sbase = smem_u32(smem_raw);
-  const uint32_t sW = sbase + oW, sT = sbase + oT, sBar = sbase + oBar;
-  float* const s_b = reinterpret_cast<float*>(smem_raw + oPar);       // ln_b | b2
+  const uint32_t sW = sbase + L::W, sT = sbase + L::T, sBar = sbase + L::Bar;
+  float* const s_b = reinterpret_cast<float*>(smem_raw + L::Par);       // ln_b | b2
   float* const s_b2 = s_b + 128;
   // the warp index is broadcast from lane 0 so that the compiler knows it is warp-uniform
   const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
@@ -164,7 +188,9 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   if ((sbase & 1023u) != 0) __trap();            // SWIZZLE_128B atoms need a 1024-byte aligned window
   if (d_counts) { n_dst = d_counts[0]; split_dst = d_counts[1]; }      // destination subset compacted on the device
   const long long n_rows = n_dst * k, split_rows = split_dst * k;      // both multiples of 128 by construction of the lists
-  const long long n_tiles = (n_rows + kTile - 1) / kTile;
+  long long row_lo = 0, row_hi = n_rows;                               // the launch's rows: one class for FOLD, else all
+  if constexpr (FOLD) { if (fold_cls) row_lo = split_rows; else row_hi = split_rows; }
+  const long long n_tiles = row_hi > row_lo ? (row_hi - row_lo + kTile - 1) / kTile : 0;
   const long long my_tiles = (n_tiles > blockIdx.x) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
   // P stage c: full[c] (producer -> consumer c, 32 producer lanes + the bytes of the copies), empty[c] (consumer c's 128 threads)
   auto full_bar = [&](int c) { return sBar + 8u * (1 + c); };
@@ -177,9 +203,15 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
     mbar_init(sBar, 1);
     for (int c = 0; c < kCons; ++c) { mbar_init(full_bar(c), 32); mbar_init(empty_bar(c), 128); }
     fence_barrier_init();
-    mbar_expect_tx(sBar, 2u * kWPiece + 2u * kTabClassBytes);
-    bulk_g2s(sW, w2_image, 2u * kWPiece, sBar);
-    bulk_g2s(sT, tab_image, 2u * kTabClassBytes, sBar);
+    if constexpr (FOLD) {                       // W2^T fp32 (the same 64 KB as the two bf16 pieces) and this launch's class table
+      mbar_expect_tx(sBar, 4u * 128 * 128 + kTabClassBytes);
+      bulk_g2s(sW, w2_image, 4u * 128 * 128, sBar);
+      bulk_g2s(sT, tab_image + (size_t)fold_cls * kTabClassBytes, kTabClassBytes, sBar);
+    } else {
+      mbar_expect_tx(sBar, 2u * kWPiece + 2u * kTabClassBytes);
+      bulk_g2s(sW, w2_image, 2u * kWPiece, sBar);
+      bulk_g2s(sT, tab_image, 2u * kTabClassBytes, sBar);
+    }
   }
   for (int i = tid; i < 128; i += kThreads) { s_b[i] = lp.b[i]; s_b2[i] = lp.b2[i]; }
   __syncthreads();
@@ -191,13 +223,13 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
     // copies remain between the consumer's hand-back and its next tile.
     if (warp >= kCons) return;
     const int c = warp;
-    const uint32_t st = sbase + oStage + (uint32_t)c * kStage;
+    const uint32_t st = sbase + L::Stage + (uint32_t)c * kStage;
     for (long long it = c, use = 0; it < my_tiles; it += kCons, ++use) {
-      const long long tile = blockIdx.x + it * (long long)gridDim.x, row0 = tile * kTile;
+      const long long tile = blockIdx.x + it * (long long)gridDim.x, row0 = row_lo + tile * kTile;
       int j0;
       const unsigned a0 = row_dst(row0, j0);
-      const long long last = (row0 + kTile - 1 < n_rows ? row0 + kTile - 1 : n_rows - 1);
-      const int n_d = min(kDst, (int)(row_dst(last, j0) - a0) + 1);   // destinations with a staged P[dst] row
+      const long long last = (row0 + kTile - 1 < row_hi ? row0 + kTile - 1 : row_hi - 1);
+      const int n_d = min(kDst, (int)(row_dst(last, j0) - a0) + 1);   // destinations with a staged P[dst] row (FOLD: at most 2, + q rows)
       int s[2];
       int4 meta[2];
 #pragma unroll
@@ -221,14 +253,16 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       if (lane < n_d) dnode = row_nodes[a0 + lane];
       mbar_wait(empty_bar(c), (uint32_t)(use & 1) ^ 1u);              // the first use of a stage passes at once
 #pragma unroll
-      for (int h = 0; h < 2; ++h) *reinterpret_cast<int4*>(smem_raw + oStage + c * kStage + sMeta + 16 * (lane + 32 * h)) = meta[h];
-      if (lane == 0) mbar_expect_tx_only(full_bar(c), (uint32_t)(kTile + n_d) * 512u);
+      for (int h = 0; h < 2; ++h) *reinterpret_cast<int4*>(smem_raw + L::Stage + c * kStage + sMeta + 16 * (lane + 32 * h)) = meta[h];
+      if (lane == 0) mbar_expect_tx_only(full_bar(c), (uint32_t)(kTile + (FOLD ? 2 : 1) * n_d) * 512u);
       __syncwarp();
       // absent slots read the all-zero row `zero_row` kept by the engine
 #pragma unroll
       for (int h = 0; h < 2; ++h)
         bulk_g2s(st + sSrc + (uint32_t)(lane + 32 * h) * kSrcStride, P + (size_t)(s[h] >= 0 ? s[h] : zero_row) * TD_NPROJ + offB, 512u, full_bar(c));
       if (lane < n_d) bulk_g2s(st + sDstRows + (uint32_t)lane * 512u, P + (size_t)(dnode >= 0 ? dnode : zero_row) * TD_NPROJ + offA, 512u, full_bar(c));
+      // FOLD: q[dst] rows in P[dst] slots 2 + lane (a padding destination, which has no valid edge: row 0)
+      if (FOLD && lane < n_d) bulk_g2s(st + sDstRows + (uint32_t)(2 + lane) * 512u, qnode + (size_t)(dnode >= 0 ? dnode : 0) * TD_H, 512u, full_bar(c));
       mbar_arrive(full_bar(c));
     }
     return;
@@ -245,11 +279,19 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
 
   const int r_base = 16 * w + (lane >> 2);
   const int pair_bar = 1 + 2 * cwg + (w >> 1);                  // named barrier of the warp pair {w & 2, (w & 2) + 1}
-  float* const xslot = reinterpret_cast<float*>(smem_raw + oX) + (size_t)(cwg * 4 + w) * 256;   // 2 sets x 128; partner at (w ^ 1)
+  float* const xslot = reinterpret_cast<float*>(smem_raw + L::X) + (size_t)(cwg * 4 + w) * 256;   // 2 sets x 128; partner at (w ^ 1)
   float* const xpart = xslot + ((w & 1) ? -256 : 256);
-  const bool do_agg = NOUT == 128 && qnode == nullptr && agg.logits != nullptr;
+  const bool do_agg = !FOLD && NOUT == 128 && qnode == nullptr && agg.logits != nullptr;
   const bool key_sm = NOUT == 128 && qnode != nullptr && agg.key_softmax;
-  const unsigned char* const stage = smem_raw + oStage + cwg * kStage;
+  const unsigned char* const stage = smem_raw + L::Stage + cwg * kStage;
+  // FOLD: this thread builds M rows of head fhd (both slots) over K runs frun and frun + 8 (8 f each).  In a quarter warp the W2
+  // reads (first half fs of the head's 8 values) and the 16-byte image stores each fall in 8 distinct bank groups.
+  const int ct = tid & 127, fu = ct & 7, fg = ct >> 3;
+  const int fhd = 8 * (fg & 1) + 4 * (fu >> 2) + (fu & 3), fs = fu >> 2, frun = (fg >> 1) ^ (((fu >> 1) & 1) << 2);
+  const int fn0 = 16 * ((fhd >> 1) & 1) + 2 * (fhd >> 2) + (fhd & 1);         // M row of (head fhd, slot 0); slot 1 is fn0 + 8
+  unsigned char* const mimg = smem_raw + L::M + cwg * kMImg;
+  float* const s_c = reinterpret_cast<float*>(smem_raw + L::C) + cwg * 32;      // c_dst[slot][head]
+  const int srow = k == 32 ? (w >> 1) : 0;                                        // FOLD: destination slot of this warp's rows
   // MMA phase order: consumer 0 first, then strictly alternating.  Every consumer runs the same number of iterations (one without
   // a tile only passes the order on); consumer 1's first hand-over and consumer 0's wait after the loop keep the counts equal, so
   // no barrier is left half-arrived.
@@ -265,8 +307,8 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       for (int phase = 0; phase < 2; ++phase) { named_bar_sync(order_mine, 256); named_bar_arrive(order_other, 256); }
       continue;
     }
-    const long long tile = blockIdx.x + it * (long long)gridDim.x;
-    const int cls = (tile * kTile >= split_rows) ? 1 : 0;
+    const long long tile = blockIdx.x + it * (long long)gridDim.x, row0 = row_lo + tile * kTile;
+    const int cls = FOLD ? 0 : (row0 >= split_rows) ? 1 : 0;       // FOLD: the one resident table
     // ---- metadata of this thread's two rows (s < 0: absent edge / padding destination / beyond the end)
     long long idx[2];
     int node[2], s[2], ty[2], jj[2], dsl[2];
@@ -274,10 +316,30 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
     mbar_wait(full_bar(cwg), (uint32_t)(n & 1));
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      idx[h] = tile * kTile + r_base + 8 * h;
+      idx[h] = row0 + r_base + 8 * h;
       const int4 m4 = *reinterpret_cast<const int4*>(stage + sMeta + 16 * (r_base + 8 * h));
       node[h] = m4.x; s[h] = m4.y; dist[h] = __int_as_float(m4.z);
       ty[h] = m4.w & 0xff; dsl[h] = ((m4.w >> 8) & 0xff) - 1; jj[h] = m4.w >> 16;
+    }
+    // ---- FOLD: the edge gates (used after the main MMA) and this thread's q rows, times 1/sqrt(8), in the order its W2 reads take
+    //      (half fs first); slot 1 is zero when a tile is one destination (k = 64)
+    float ewp[2] = {0.f, 0.f};
+    float4 qf[2][2];
+    if constexpr (FOLD) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (key_sm && idx[h] < n_rows && node[h] >= 0) ewp[h] = agg.e_w[(size_t)node[h] * k + jj[h]];
+#pragma unroll
+      for (int sl = 0; sl < 2; ++sl)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (sl == 0 || k == 32) {
+            v = *reinterpret_cast<const float4*>(stage + sDstRows + (2 + sl) * 512 + 32 * fhd + 16 * (hf ^ fs));
+            v.x *= 0.35355339059327373f; v.y *= 0.35355339059327373f; v.z *= 0.35355339059327373f; v.w *= 0.35355339059327373f;
+          }
+          qf[sl][hf] = v;
+        }
     }
     // ---- G in the A fragment: K-slot half 0 = edge from a protein atom (types 3 / 2), half 1 = from a ligand atom (types 1 / 0).
     //      Inside the row's half, this lane's slots (kk, register) carry m = 4 (kk % 2) + 2 (register / 2) + {0, 1}: gaussian 5 q + m
@@ -338,6 +400,52 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
     }
     wgmma_commit();
     named_bar_arrive(order_other, 256);
+    if constexpr (FOLD) {
+      // ---- while the pre-MMA runs: M rows fn0 (slot 0) and fn0 + 8 (slot 1) over this thread's two K runs, split into two bf16
+      //      pieces and stored in the K-major SWIZZLE_128B image (the previous tile's main MMA has completed in every warp: they all
+      //      passed the order barrier above).  Per f the two halves are summed apart, so the value does not depend on fs.
+      const float* const w2s = reinterpret_cast<const float*>(smem_raw + L::W) + 8 * fhd;
+#pragma unroll
+      for (int jr = 0; jr < 2; ++jr) {
+        const int f0 = 64 * jr + 8 * frun;
+        float mv[2][8];
+#pragma unroll
+        for (int jf = 0; jf < 8; ++jf) {
+          const float4 wa = *reinterpret_cast<const float4*>(w2s + (f0 + jf) * 128 + 4 * fs);
+          const float4 wb = *reinterpret_cast<const float4*>(w2s + (f0 + jf) * 128 + 4 * (fs ^ 1));
+#pragma unroll
+          for (int sl = 0; sl < 2; ++sl) {
+            const float4 qa = qf[sl][0], qb = qf[sl][1];
+            const float pa = __fmaf_rn(wa.w, qa.w, __fmaf_rn(wa.z, qa.z, __fmaf_rn(wa.y, qa.y, wa.x * qa.x)));
+            const float pb = __fmaf_rn(wb.w, qb.w, __fmaf_rn(wb.z, qb.z, __fmaf_rn(wb.y, qb.y, wb.x * qb.x)));
+            mv[sl][jf] = pa + pb;
+          }
+        }
+#pragma unroll
+        for (int sl = 0; sl < 2; ++sl) {
+          uint4 hi, lo;
+          split2(mv[sl][0], mv[sl][1], hi.x, lo.x);
+          split2(mv[sl][2], mv[sl][3], hi.y, lo.y);
+          split2(mv[sl][4], mv[sl][5], hi.z, lo.z);
+          split2(mv[sl][6], mv[sl][7], hi.w, lo.w);
+          const int nr = fn0 + 8 * sl;
+          const int off = jr * kMAtom + (nr >> 3) * 1024 + (nr & 7) * 128 + ((frun ^ (nr & 7)) << 4);
+          *reinterpret_cast<uint4*>(mimg + off) = hi;
+          *reinterpret_cast<uint4*>(mimg + kMPiece + off) = lo;
+        }
+      }
+      // c_dst (one thread per head)
+      if (fg < 2)
+#pragma unroll
+        for (int sl = 0; sl < 2; ++sl) {
+          const float4 ba = *reinterpret_cast<const float4*>(s_b2 + 8 * fhd + 4 * fs), bb = *reinterpret_cast<const float4*>(s_b2 + 8 * fhd + 4 * (fs ^ 1));
+          const float4 qa = qf[sl][0], qb = qf[sl][1];
+          const float pa = __fmaf_rn(ba.w, qa.w, __fmaf_rn(ba.z, qa.z, __fmaf_rn(ba.y, qa.y, ba.x * qa.x)));
+          const float pb = __fmaf_rn(bb.w, qb.w, __fmaf_rn(bb.z, qb.z, __fmaf_rn(bb.y, qb.y, bb.x * qb.x)));
+          s_c[16 * sl + fhd] = pa + pb;
+        }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the image is read by wgmma (async proxy)
+    }
     wgmma_wait_all();
     // ---- LayerNorm over the 128 features of each row (centred by the packer: the variance is the mean square): 32 per lane, the 4
     //      lanes of the quad combine by shuffles
@@ -367,17 +475,34 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
         const float y0 = __fmaf_rn(x[e], rstd[h], b.x), y1 = __fmaf_rn(x[e + 1], rstd[h], b.y);
         split2(fmaxf(y0, 0.f), fmaxf(y1, 0.f), ahi[kk][r], alo[kk][r]);
       }
-    // ---- D = hid . W2^T
+    // ---- D = hid . W2^T   (FOLD: D = c_dst + hid . M^T, N = 32; o[4 i + 2 h + c] is head 4 q + 2 (i / 2) + c of slot i % 2)
     float o[NOUT / 2];
+    if constexpr (FOLD) {
+      named_bar_sync(kFoldBar + cwg, 128);                          // M image and c_dst written by all 4 warps
+#pragma unroll
+      for (int sl = 0; sl < 2; ++sl) {
+        const float4 cv = *reinterpret_cast<const float4*>(s_c + 16 * sl + 4 * q);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          o[4 * sl + 2 * h] = cv.x; o[4 * sl + 2 * h + 1] = cv.y;
+          o[4 * (2 + sl) + 2 * h] = cv.z; o[4 * (2 + sl) + 2 * h + 1] = cv.w;
+        }
+      }
+    }
     wgmma_fence();
     named_bar_sync(order_mine, 256);
 #pragma unroll
     for (int term = 0; term < 3; ++term) {
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk) {
-        const uint64_t desc = gmma_desc_sw128(sW + (term == 1 ? kWPiece : 0) + (kk >> 2) * kWAtom + (kk & 3) * 32);
-        if constexpr (NOUT == 128) wgmma_n128_rs(o, term == 2 ? alo[kk] : ahi[kk], desc, (term | kk) ? 1u : 0u);
-        else wgmma_n16_rs(o, term == 2 ? alo[kk] : ahi[kk], desc, (term | kk) ? 1u : 0u);
+        if constexpr (FOLD) {
+          const uint64_t desc = gmma_desc_sw128(sbase + L::M + cwg * kMImg + (term == 1 ? kMPiece : 0) + (kk >> 2) * kMAtom + (kk & 3) * 32);
+          wgmma_n32_rs(reinterpret_cast<float(&)[16]>(o), term == 2 ? alo[kk] : ahi[kk], desc, 1u);
+        } else {
+          const uint64_t desc = gmma_desc_sw128(sW + (term == 1 ? kWPiece : 0) + (kk >> 2) * kWAtom + (kk & 3) * 32);
+          if constexpr (NOUT == 128) wgmma_n128_rs(o, term == 2 ? alo[kk] : ahi[kk], desc, (term | kk) ? 1u : 0u);
+          else wgmma_n16_rs(o, term == 2 ? alo[kk] : ahi[kk], desc, (term | kk) ? 1u : 0u);
+        }
       }
     }
     wgmma_commit();
@@ -444,7 +569,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
         const float2 a = *reinterpret_cast<const float2*>(se + ccol), b = *reinterpret_cast<const float2*>(so + ccol);
         *reinterpret_cast<float2*>(agg.h + (size_t)dnode * TD_H + ccol) = make_float2(hin.x + (a.x + b.x), hin.y + (a.y + b.y));
       }
-    } else if (qnode == nullptr) {
+    } else if (!FOLD && qnode == nullptr) {
       // ---- value MLPs: out[row, :] = D + b2
 #pragma unroll
       for (int h = 0; h < 2; ++h)
@@ -459,20 +584,31 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       //      (reference models/uni_transformer.py:73,135): head hd is fragment column block i = hd; 2 products per lane, then the quad.
       //      lg[4 h + u] (after the quad reduction) = head 4 q + u of row h.
       float lg[32];
+      if constexpr (FOLD) {
+        // the logits are the D fragment itself: this row's slot srow, heads 4 q + 2 jb + c in o[4 (2 jb + srow) + 2 h + c]
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float* qrow = qnode + (size_t)(node[h] >= 0 ? node[h] : 0) * TD_H + 2 * q;
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float2 qv = __ldg(reinterpret_cast<const float2*>(qrow + 8 * i));
-          const float2 bb = *reinterpret_cast<const float2*>(s_b2 + 8 * i + 2 * q);
-          // element order for the reduction over the quad: 8 (i / 4) + 4 h + i % 4 -> lane q keeps heads 4 q ..
-          lg[8 * (i >> 2) + 4 * h + (i & 3)] = __fmaf_rn(o[4 * i + 2 * h + 1] + bb.y, qv.y, (o[4 * i + 2 * h] + bb.x) * qv.x);
+          for (int u = 0; u < 4; ++u) {
+            const int e0 = 4 * (2 * (u >> 1)) + 2 * h + (u & 1);
+            lg[4 * h + u] = srow ? o[e0 + 4] : o[e0];
+          }
+      } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float* qrow = qnode + (size_t)(node[h] >= 0 ? node[h] : 0) * TD_H + 2 * q;
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const float2 qv = __ldg(reinterpret_cast<const float2*>(qrow + 8 * i));
+            const float2 bb = *reinterpret_cast<const float2*>(s_b2 + 8 * i + 2 * q);
+            // element order for the reduction over the quad: 8 (i / 4) + 4 h + i % 4 -> lane q keeps heads 4 q ..
+            lg[8 * (i >> 2) + 4 * h + (i & 3)] = __fmaf_rn(o[4 * i + 2 * h + 1] + bb.y, qv.y, (o[4 * i + 2 * h] + bb.x) * qv.x);
+          }
         }
-      }
-      transpose_reduce<32, 8, 0>(lg, lane);
+        transpose_reduce<32, 8, 0>(lg, lane);
 #pragma unroll
-      for (int u = 0; u < 8; ++u) lg[u] *= 0.35355339059327373f;          // 1/sqrt(8)
+        for (int u = 0; u < 8; ++u) lg[u] *= 0.35355339059327373f;          // 1/sqrt(8)
+      }
       if (key_sm) {
         // softmax over the destination's 32 edges (the warp pair's rows) for this lane's 4 heads, times the edge gate: the value
         // launch's epilogue only has to weight and sum.
@@ -483,7 +619,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
           valid_e[h] = false; ew[h] = 0.f;
           if (owrite[h]) {
             valid_e[h] = s[h] >= 0;
-            ew[h] = agg.e_w[(size_t)node[h] * k + jj[h]];
+            ew[h] = FOLD ? ewp[h] : agg.e_w[(size_t)node[h] * k + jj[h]];
           }
         }
         float mx[4], sm[4];
@@ -542,16 +678,32 @@ void td_launch_edge_mlp_v4(const float* P, int zero_row, const int* src, const u
   memset(lp.b2, 0, sizeof(lp.b2));
   memcpy(lp.b2, h_b2, sizeof(float) * (size_t)m.nout);
   memcpy(lp.mu, h_offsets, sizeof(lp.mu));
-  static size_t opted128[TD_MAX_DEVICES] = {0}, opted16[TD_MAX_DEVICES] = {0};
-  td_opt_in_smem(edge_mlp_v4_kernel<128>, kSmem, opted128);
-  td_opt_in_smem(edge_mlp_v4_kernel<16>, kSmem, opted16);
-  const long long n_tiles = (n_dst * k + kTile - 1) / kTile;         // with d_counts: upper bound
-  const int grid = (int)(n_tiles < sm_count ? n_tiles : sm_count);
+  static size_t opted128[TD_MAX_DEVICES] = {0}, opted16[TD_MAX_DEVICES] = {0}, optedF[TD_MAX_DEVICES] = {0};
+  td_opt_in_smem(edge_mlp_v4_kernel<128, false>, Map<false>::Smem, opted128);
+  td_opt_in_smem(edge_mlp_v4_kernel<16, false>, Map<false>::Smem, opted16);
+  td_opt_in_smem(edge_mlp_v4_kernel<128, true>, Map<true>::Smem, optedF);
+  auto grid_of = [&](long long n_dst_range) {                         // with d_counts: upper bound
+    const long long n_tiles = (n_dst_range * k + kTile - 1) / kTile;
+    return (int)(n_tiles < sm_count ? n_tiles : sm_count);
+  };
   AggArgs agg = {agg_logits, agg_e_w, agg_h, (key_softmax && k == 32) ? 1 : 0};
-  if (m.nout == 16)
-    edge_mlp_v4_kernel<16><<<grid, kThreads, kSmem, st>>>(P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB, m.w2_img,
-                                                         m.tabcls_img, coeff, nullptr, out, out_by_slot, agg, lp);
-  else
-    edge_mlp_v4_kernel<128><<<grid, kThreads, kSmem, st>>>(P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB, m.w2_img,
-                                                          m.tabcls_img, coeff, qnode, out, out_by_slot, agg, lp);
+  if (m.nout == 16) {
+    edge_mlp_v4_kernel<16, false><<<grid_of(n_dst), kThreads, Map<false>::Smem, st>>>(
+        P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB, m.w2_img, m.tabcls_img, coeff, nullptr, out,
+        out_by_slot, agg, 0, lp);
+  } else if (qnode && (k == 32 || k == 64)) {
+    // folded key launch, one per destination class (a tile then holds at most 2 destinations); the host split bounds the device one
+    // from above and the ligand part is the same on both, so a class the host counts as empty is empty on the device too
+    const long long n_cls[2] = {split_dst, n_dst - split_dst};
+    for (int cls = 0; cls < 2; ++cls)
+      if (n_cls[cls] > 0)
+        edge_mlp_v4_kernel<128, true><<<grid_of(n_cls[cls]), kThreads, Map<true>::Smem, st>>>(
+            P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB,
+            reinterpret_cast<const unsigned char*>(m.w2t), m.tabcls_img, coeff, qnode, out, out_by_slot, agg, cls, lp);
+  } else {
+    // k <= 31 or k = 48: a tile spans more destinations than the N = 32 fold has slots for; keys are computed whole
+    edge_mlp_v4_kernel<128, false><<<grid_of(n_dst), kThreads, Map<false>::Smem, st>>>(
+        P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB, m.w2_img, m.tabcls_img, coeff, qnode, out,
+        out_by_slot, agg, 0, lp);
+  }
 }
