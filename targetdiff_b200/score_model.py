@@ -300,7 +300,11 @@ class ScorePosNet3D(nn.Module):
         if self.time_emb_dim > 0:           # (time_step / T) per graph, fp32 like the reference's true division (:322)
             if time_step is None:
                 raise ValueError('time_step is required when time_emb_dim > 0')
-            tn = (time_step.to(dev) / self.num_timesteps).to(torch.float32).contiguous()
+            # divided by a tensor, not a Python number: torch's CUDA division by a scalar multiplies by the rounded reciprocal, which
+            # is one ulp off the correctly rounded t / T for some t (9, 13, 18 of T = 20); the sampling chain's set_time_kernel and
+            # the CPU oracle divide
+            tn = time_step.to(dev, torch.float32)
+            tn = (tn / torch.full_like(tn, float(self.num_timesteps))).contiguous()
             if tn.numel() != B:
                 raise ValueError('time_step must have one entry per graph')
             _lib.check(lib.tdiff_set_time(eng, _ptr(tn), st))

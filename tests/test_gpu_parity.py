@@ -240,7 +240,7 @@ def test_chain_philox_reproducible_and_sane():
     assert not torch.equal(r1['pos'], r3['pos'])
     assert torch.isfinite(r1['pos']).all() and int(r1['v'].min()) >= 0 and int(r1['v'].max()) < 13
     assert len(r1['pos_traj']) == 12 and r1['pos_traj'][0].shape == (50, 3)
-    # device noise has the right moments: the one-step position noise is N(0, sigma_t^2)
+    # the device stream itself (its values and its distribution): tests/test_gpu_sampler.py
     lp = torch.stack(r1['vt_traj'])
     torch.testing.assert_close(lp.exp().sum(-1), torch.ones(12, 50), rtol=0, atol=1e-4)
 
