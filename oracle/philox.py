@@ -82,3 +82,30 @@ def engine_tape(seed, n_lig, num_steps, K, pos_only=False):
     else:
         vu = type_uniforms(seed, a, s, K).astype(np.float32)
     return torch.from_numpy(pn), torch.from_numpy(vu)
+
+
+# A chain run with `seed=` against the same chain on `engine_tape(seed, ...)`, limits about 3-4x the largest value measured on one
+# NVIDIA H100 80GB HBM3 at a 400 W power limit.  First step: |pos_seed - pos_tape| in fp32 ulps of (|pos| + sigma |noise|), measured
+# at most 0.83.  Later steps: max |pos_seed - pos_tape| relative to the largest coordinate of the step (the network carries the first
+# step's ulps forward), measured at most 7.5e-8.
+STREAM_ULPS, STREAM_LATER_REL = 3.0, 3e-7
+
+
+def stream_errors(pos_seed, pos_tape, pos_noise0, sigma0, offset=None):
+    """(first-step error in ulps, later steps' relative error) of the position trajectories [S, Nl, 3] of a seeded chain and of the
+    same chain on its engine_tape, whose first step has the noise `pos_noise0` [Nl, 3] and sigma `sigma0`.  With the centring
+    `offset` [Nl, 3] (center_pos_mode='protein'), the step's position is a sum in the centred frame to which the offset is added, so
+    the ulps are of |pos| + |pos - offset| + sigma |noise|: where pos nearly cancels the offset, the centred sum's rounding is
+    larger than an ulp of pos."""
+    eps32 = 2.0 ** -23
+    p0 = pos_tape[0].double()
+    d0 = (pos_seed[0].double() - p0).abs()
+    scale = p0.abs() + sigma0 * pos_noise0.double().abs()
+    if offset is not None:
+        scale = scale + (p0 - offset.double()).abs()
+    ulps = float((d0 / (eps32 * scale)).max())
+    later = 0.0
+    if pos_seed.shape[0] > 1:
+        dl = (pos_seed[1:] - pos_tape[1:]).abs().flatten(1).amax(1)
+        later = float((dl / pos_tape[1:].abs().flatten(1).amax(1)).max())
+    return ulps, later

@@ -25,19 +25,7 @@ pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
 MODE_ID = {'simt': 0, 'tc3v2': 2, 'tc6': 3, 'tc3': 5}
 POS_RTOL, POS_ATOL, LOGIT_ATOL, H_RTOL, H_ATOL = 1e-4, 1e-5, 1e-3, 1e-4, 1e-4
-
-# Largest per-row error (h, x) of one layer against float64 allowed per edge-MLP mode, about 3-4x the maximum measured on one
-# NVIDIA H100 80GB HBM3 at a 400 W power limit (the kernels are deterministic).  The fp32 oracle's own error on the same inputs is
-# 3e-7 - 9e-7 in h and up to 1.8e-4 in x.  Measured maxima, and the cases they cover:
-#   every mode, k = 8, 32, 48 (test_layer_parity_every_mode):  tc3 h 8.7e-6 x 1.4e-4 | tc3v2 h 8.1e-6 x 8.6e-5 |
-#                                                               tc6 h 2.5e-6 x 3.1e-5 | simt  h 5.7e-7 x 2.4e-5
-#   tc3 (default), every other case of this file, k >= 2:      h 1.22e-5 (x2h_out_fc)   x 8.9e-4 (the 40-graph batch, 1600 ligand rows)
-#   tc3, k = 1:                                                h 1.27e-5                 x 1.53e-3
-# The bf16-split modes keep ~16 mantissa bits per operand, hence ~1e-5 in h.  x is relative to the layer's displacement, a mean
-# over 16 heads of signed terms (at k = 1, of one edge's terms only): rows where they nearly cancel amplify every mode's error, the
-# fp32 oracle's too.  The k = 1 maximum gets its own x limit so that it does not loosen the check at every other k.
-LAYER_TOL = {'tc3': (4e-5, 3e-3), 'tc3v2': (3e-5, 3e-4), 'tc6': (1e-5, 1e-4), 'simt': (2e-6, 8e-5)}
-X_TOL_K1 = 5e-3                                        # tc3, k = 1
+# per-layer limits against float64 (LAYER_TOL, X_TOL_K1) and the measured maxima behind them: oracle/layerwise.py
 
 EDGE_MLPS = ('.hk_func.', '.hv_func.', '.xk_func.', '.xv_func.')
 
@@ -98,58 +86,19 @@ def _args(b, dev=DEV):
     return tuple(b[k].to(dev) for k in ('protein_pos', 'protein_v', 'batch_protein', 'init_ligand_pos', 'init_ligand_v', 'batch_ligand'))
 
 
-def _sorted_edges(ei):
-    key = ei[1] * (int(ei.max()) + 1 if ei.numel() else 1) + ei[0]
-    return ei[:, torch.argsort(key)]
-
-
 # ------------------------------------------------------------------------------------------------ 1. layer by layer vs float64
 def _layer_parity(label, cfg, sd, b, n_layers, mode='tc3', time_step=None):
-    """Runs prefixes of 1..n_layers layers; returns [(layer, h err max, h p99.9, x err max, x p99.9, fp32 oracle's 4 values)]."""
-    cfg = dict(cfg or {})
-    pp, lp, _ = restate.center_pos(b['protein_pos'], b['init_ligand_pos'], b['batch_protein'], b['batch_ligand'])
-    tr = {}
-    restate.forward(sd, dict(cfg, num_layers=1), pp, b['protein_v'], b['batch_protein'], lp, b['init_ligand_v'], b['batch_ligand'],
-                    trace=tr, time_step=time_step)
-    ref64 = layerwise.LayerRef.from_trace(sd, cfg, tr)
-    ref32 = layerwise.LayerRef.from_trace(sd, cfg, tr, dtype=torch.float32)
-    lig = tr['mask_ligand']
-    hybrid = cfg.get('cutoff_mode') == 'hybrid'
-    args = (pp.to(DEV), b['protein_v'].to(DEV), b['batch_protein'].to(DEV), lp.to(DEV), b['init_ligand_v'].to(DEV), b['batch_ligand'].to(DEV))
-    kw = {} if time_step is None else {'time_step': time_step.to(DEV)}
-    h, x = tr['all_h'][0], tr['all_x'][0]
-    rows = []
-    for l in range(1, n_layers + 1):
-        model = _model(dict(cfg, num_layers=l), layerwise.prefix_state_dict(sd, l))
-        out = model(*args, **kw)
-        if l == 1:
-            from targetdiff_b200 import _lib
-            assert _lib.load().tdiff_edge_mlp_mode(model.engine(DEV)) == MODE_ID[mode]
-        ei = out['edge_index'].cpu()
-        if hybrid:              # the engine's slot list is destination-sorted; the edge set must agree bit for bit
-            assert torch.equal(_sorted_edges(ei), _sorted_edges(tr['edge_index']))
-        else:
-            assert torch.equal(ei, tr['edge_index'])
-        h_gpu = out['final_h'].cpu()
-        x_gpu = x.clone()
-        x_gpu[lig] = out['pred_ligand_pos'].cpu()
-        h64, x64 = ref64(l - 1, h, x)
-        h32, x32 = ref32(l - 1, h, x)
-        r = (l,) + layerwise.summary(layerwise.row_error(h_gpu, h64, h)) + layerwise.summary(layerwise.row_error(x_gpu, x64, x, lig)) + \
-            layerwise.summary(layerwise.row_error(h32, h64, h)) + layerwise.summary(layerwise.row_error(x32, x64, x, lig))
-        rows.append(r)
-        print('%-28s %-6s layer %d  h %.2e / %.2e  x %.2e / %.2e   fp32 oracle: h %.2e / %.2e  x %.2e / %.2e' % ((label, mode) + r))
-        h, x = h_gpu, x_gpu
-        del model
-    return rows
+    """Runs prefixes of 1..n_layers layers (oracle.layerwise.engine_layer_parity), each in edge-MLP mode `mode`; returns
+    [(layer, h err max, h p99.9, x err max, x p99.9, fp32 oracle's 4 values)]."""
+    def make(c, s):
+        from targetdiff_b200 import _lib
+        model = _model(c, s)
+        assert _lib.load().tdiff_edge_mlp_mode(model.engine(DEV)) == MODE_ID[mode]
+        return model
+    return layerwise.engine_layer_parity(label, cfg, sd, b, n_layers, make, DEV, time_step=time_step, tag=mode)
 
 
-def _check_layers(rows, mode, k=32):
-    th, tx = LAYER_TOL[mode]
-    if k == 1:
-        tx = X_TOL_K1
-    for r in rows:
-        assert r[1] <= th and r[3] <= tx, 'layer %d: h %.3e (limit %.1e), x %.3e (limit %.1e)' % (r[0], r[1], th, r[3], tx)
+_check_layers = layerwise.check_layers
 
 
 @pytest.mark.parametrize('k', [1, 2, 7, 8, 9, 10, 16, 31, 32, 33, 48, 63, 64])

@@ -26,20 +26,9 @@ from oracle import philox, restate, stepwise, synth
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
 K = synth.LIGAND_NUM_CLASSES
-EPS32 = 2.0 ** -23
 Z_MAX, P_MIN = 5.0, 1e-6
-
-# Limits: about 3-4x the largest value measured on one NVIDIA H100 80GB HBM3 at a 400 W power limit (the kernels are deterministic),
-# or of the fp32 oracle's own error where that is larger, as in tests/test_gpu_layer_parity.py.
-# A: device stream vs engine_tape.  First step: |pos_seed - pos_tape| in fp32 ulps of (|pos| + sigma |noise|), measured at most 0.83.
-# Later steps: max |pos_seed - pos_tape| relative to the largest coordinate of the step (the network carries the first step's ulps
-# forward), measured at most 7.5e-8.
-STREAM_ULPS, STREAM_LATER_REL = 3.0, 3e-7
-# B: per-step errors against float64.  Measured maxima, engine / fp32 oracle: position (relative) 1.39e-7 / 1.65e-7, v0 (absolute)
-# 4.1e-7 / 3.8e-7, vt (absolute) 1.94e-6 / 1.70e-6.  The position error is 0 at t = 0 for both (sigma = 0 and x0 enters exactly).
-STEP_TOL = {'pos': 6e-7, 'v0': 1.5e-6, 'vt': 6e-6}
-# atoms whose float64 Gumbel margin (best score minus runner-up) is at most MARGIN are not compared; none occurred in any case
-MARGIN, MAX_EXEMPT = 1e-4, 2
+# Limits of A (philox.STREAM_ULPS, STREAM_LATER_REL) and B (stepwise.STEP_TOL), with the measured maxima behind them: oracle/philox.py
+# and oracle/stepwise.py.
 
 
 def _model(cfg=None, weight_seed=0):
@@ -83,14 +72,9 @@ def _stream_case(setup, seed, S, pos_only):
     else:
         assert torch.equal(dev['v0_traj'][0], tape['v0_traj'][0]) and torch.equal(dev['vt_traj'][0], tape['vt_traj'][0])
     T = sd['betas'].shape[0]
-    d0 = (dev['pos_traj'][0].double() - tape['pos_traj'][0].double()).abs()
-    ulps = float((d0 / (EPS32 * (tape['pos_traj'][0].double().abs() + _sigma(sd, T - 1) * pn[0].double().abs()))).max())
-    later = 0.0
-    if S > 1:
-        dl = (dev['pos_traj'][1:] - tape['pos_traj'][1:]).abs().flatten(1).amax(1)
-        later = float((dl / tape['pos_traj'][1:].abs().flatten(1).amax(1)).max())
+    ulps, later = philox.stream_errors(dev['pos_traj'], tape['pos_traj'], pn[0], _sigma(sd, T - 1))
     print('stream seed=%-20d S=%d pos_only=%d  step 0: %.2f ulp  later steps: %.2e rel' % (seed, S, pos_only, ulps, later))
-    assert ulps <= STREAM_ULPS and later <= STREAM_LATER_REL, (ulps, later)
+    assert ulps <= philox.STREAM_ULPS and later <= philox.STREAM_LATER_REL, (ulps, later)
 
 
 @pytest.mark.parametrize('S', [1, 2, 3, 7])
@@ -117,35 +101,10 @@ def _centred_batch(seed, sizes, n_protein=60):
 
 def _steps_vs_float64(label, cfg, S, check, pos_only=False, seed=41):
     model, sd = _model(cfg)
-    T = sd['betas'].shape[0]
     b = _centred_batch(seed, [9, 14])
-    B, n = 2, len(b['batch_ligand'])
-    pn, vu = synth.make_tape(seed, S, n)
-    r = model.sample_diffusion(*_args(b), num_steps=S, center_pos_mode='none', pos_only=pos_only, noise_tape=(pn, vu), stack_traj=True)
-    time_emb = (cfg or {}).get('time_emb_dim', 0) > 0
-    rows = []
-    for s in check:
-        t = T - 1 - s
-        xt = b['init_ligand_pos'] if s == 0 else r['pos_traj'][s - 1]
-        vt = b['init_ligand_v'] if s == 0 else r['v_traj'][s - 1]
-        kw = {'time_step': torch.full((B,), t, dtype=torch.long, device=DEV)} if time_emb else {}
-        out = model(b['protein_pos'].to(DEV), b['protein_v'].to(DEV), b['batch_protein'].to(DEV), xt.to(DEV), vt.to(DEV),
-                    b['batch_ligand'].to(DEV), **kw)
-        x0, logits = out['pred_ligand_pos'].cpu(), out['pred_ligand_v'].cpu()
-        args = (sd, cfg, t, xt, vt, x0, logits, pn[s], vu[s])
-        ref = stepwise.step(*args, pos_only=pos_only, dtype=torch.float64)
-        f32 = stepwise.step(*args, pos_only=pos_only)
-        e = stepwise.errors(r['pos_traj'][s], r['v_traj'][s], None if pos_only else r['v0_traj'][s],
-                            None if pos_only else r['vt_traj'][s], ref, MARGIN)
-        o = stepwise.errors(f32['pos'], f32['v'], f32['v0'], f32['vt'], ref, MARGIN)
-        rows.append((s, t, e, o))
-        print('%-22s s=%4d t=%4d  pos %.2e  v0 %.2e  vt %.2e  exempt %d   fp32 oracle: pos %.2e  v0 %.2e  vt %.2e' %
-              (label, s, t, e['pos'], e['v0'], e['vt'], e['exempt'], o['pos'], o['v0'], o['vt']))
-    for s, t, e, o in rows:
-        assert e['v_diff'] == 0, (label, s, t, e)
-        for k, lim in STEP_TOL.items():
-            assert e[k] <= lim, (label, s, t, k, e[k], lim)
-    assert sum(e['exempt'] for _, _, e, _ in rows) <= MAX_EXEMPT
+    pn, vu = synth.make_tape(seed, S, len(b['batch_ligand']))
+    rows = stepwise.engine_steps_vs_float64(label, model, sd, cfg, b, pn, vu, check, DEV, pos_only=pos_only)
+    stepwise.check_steps(label, rows)
     return rows
 
 
