@@ -64,7 +64,14 @@ typedef struct tdiff_config {
                               * a ligand destination gets every other ligand atom of its graph + its knn nearest protein atoms, protein
                               * destinations keep the k-NN over all atoms.  Needs knn + max ligand atoms per graph - 1 <= 64 slots and
                               * >= knn protein atoms per graph (checked at tdiff_bind_batch).  'radius' is a dead path in the reference */
-  int32_t reserved[2];       /* must be 0 */
+  int32_t sublayers;         /* layer form of every attention layer (models/uni_transformer.py:143-210; keys num_x2h, num_h2x, sync_twoup
+                              * of configs/training.yml:38-42).  0: the reference default, num_x2h = num_h2x = 1, sync_twoup = False;
+                              * otherwise 1 << 24 | sync_twoup << 16 | num_h2x << 8 | num_x2h, with num_x2h, num_h2x in 0..16 and
+                              * sync_twoup in 0..1.  A layer runs num_x2h feature updates in sequence on the layer's input coordinates,
+                              * then num_h2x coordinate updates, each reading the x2h output (sync_twoup = 0) or the layer's input h
+                              * (sync_twoup = 1) and the edge lengths of the coordinates the previous one moved; the layer's h is the
+                              * x2h output.  State_dict keys ...x2h_layers.i.* / ...h2x_layers.i.* for every i (TDIFF_EWEIGHT if absent) */
+  int32_t reserved[1];       /* must be 0 */
 } tdiff_config;
 
 /* One state_dict entry (reference key name, fp32, host memory).  SURVEY.md Appendix D lists the 384 keys. */
@@ -109,6 +116,13 @@ TDIFF_API int tdiff_set_time(tdiff_engine* e, const float* d_time_norm, void* st
  * d_final_h [N,128] (composed node order).  fix_x!=0 freezes coordinates (fetch_embedding, :619-631).
  * Does not modify the ligand state. */
 TDIFF_API int tdiff_forward(tdiff_engine* e, float* d_pred_pos, float* d_pred_logits, float* d_final_h, int fix_x, void* stream);
+
+/* tdiff_forward plus the per-block outputs of forward(..., return_all=True) (models/molopt_score_model.py:360-367,
+ * models/uni_transformer.py:303-327), for B = num_blocks: d_block_pos [(B+1),Nl,3] the ligand coordinates before block 0 and after
+ * every block, d_block_logits [(B+1),Nl,K] the v_inference head applied to the ligand rows of h at the same points (entry 0: the
+ * initial embeddings).  Entry B equals d_pred_pos / d_pred_logits.  Either may be NULL; the other outputs as tdiff_forward. */
+TDIFF_API int tdiff_forward_blocks(tdiff_engine* e, float* d_pred_pos, float* d_pred_logits, float* d_final_h, int fix_x, float* d_block_pos,
+                                   float* d_block_logits, void* stream);
 
 /* Graph of the most recent forward: number of edges, and edge_index as int64 [2,E] (row 0 = src/neighbour,
  * row 1 = dst/query), bit-compatible with PyG knn_graph(flow='source_to_target') (models/uni_transformer.py:280).

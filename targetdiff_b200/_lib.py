@@ -22,7 +22,7 @@ class tdiff_config(ctypes.Structure):
                 ('num_r_gaussian', ctypes.c_int32), ('num_classes', ctypes.c_int32), ('protein_feat_dim', ctypes.c_int32),
                 ('num_timesteps', ctypes.c_int32), ('model_mean_type', ctypes.c_int32), ('num_blocks', ctypes.c_int32),
                 ('ew_net_type', ctypes.c_int32), ('x2h_out_fc', ctypes.c_int32), ('time_emb', ctypes.c_int32), ('cutoff_mode', ctypes.c_int32),
-                ('reserved', ctypes.c_int32 * 2)]
+                ('sublayers', ctypes.c_int32), ('reserved', ctypes.c_int32 * 1)]
 
 
 class tdiff_tensor(ctypes.Structure):
@@ -44,6 +44,7 @@ SIGNATURES = {
     'tdiff_get_offset': (_i, [_vp, _vp, _vp]),
     'tdiff_set_time': (_i, [_vp, _vp, _vp]),
     'tdiff_forward': (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
+    'tdiff_forward_blocks': (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     'tdiff_num_edges': (_i64, [_vp, _vp]),
     'tdiff_get_edge_index': (_i, [_vp, _vp, _vp]),
     'tdiff_get_edge_weight': (_i, [_vp, _vp, _vp]),

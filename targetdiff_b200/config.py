@@ -50,8 +50,8 @@ def default_sampling_config():
 _SUPPORTED = dict(model_mean_type=('C0', 'noise'), beta_schedule=('sigmoid', 'linear', 'quad', 'const', 'jsd', 'cosine'),
                   v_beta_schedule=('cosine',), node_indicator=(True,), model_type=('uni_o2',),
                   hidden_dim=(128,), n_heads=(16,), edge_feat_dim=(4,), num_r_gaussian=(20,), act_fn=('relu',),
-                  norm=(True,), cutoff_mode=('knn', 'hybrid'), ew_net_type=('global', 'r', 'm', 'none'), num_x2h=(1,), num_h2x=(1,),
-                  x2h_out_fc=(False, True), sync_twoup=(False,))
+                  norm=(True,), cutoff_mode=('knn', 'hybrid'), ew_net_type=('global', 'r', 'm', 'none'),
+                  num_x2h=tuple(range(17)), num_h2x=tuple(range(17)), x2h_out_fc=(False, True), sync_twoup=(False, True))
 _WHY_NOT = {
     'cutoff_mode': "'radius' crashes in the reference itself (models/uni_transformer.py:278 reads an undefined self.r)",
     'model_type': "the EGNN backbone is outside the sampling path of the default model (SURVEY.md section 2)",

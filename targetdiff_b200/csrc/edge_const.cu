@@ -172,6 +172,44 @@ void td_launch_edge_geom(const float4* xm, const int* src, const unsigned char* 
   if (n > 0) edge_geom_kernel<<<(int)((n + 255) / 256), 256, 0, st>>>(xm, src, etype, n, k, dist, ew);
 }
 
+// Edge lengths of the slots of a list of destination rows (the ligand atoms), from the current coordinates, and optionally one 'r'
+// gate set sigmoid(b + sum_j w[20 type + j] g_j(dist)) for them: the reference recomputes rel_x / dist after every h2x sub-layer
+// (models/uni_transformer.py:207-208) and each h2x sub-layer has its own ew_net (:121-122).  Same arithmetic as edge_geom_kernel.
+__global__ void edge_geom_rows_kernel(const float4* __restrict__ xm, const int* __restrict__ src, const unsigned char* __restrict__ etype,
+                                      const int* __restrict__ rows, long long n_slots, int k, float* __restrict__ dist,
+                                      const float* __restrict__ gate_w, float gate_b, const float* __restrict__ offsets, float coeff,
+                                      float* __restrict__ gate) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_slots) return;
+  const long long e = (long long)rows[t / k] * k + t % k;
+  const int s = src[e];
+  float d = 0.0f;
+  if (s >= 0) {
+    const float4 xd = xm[e / k], xs = xm[s];
+    const float dx = xd.x - xs.x, dy = xd.y - xs.y, dz = xd.z - xs.z;
+    d = sqrtf(dx * dx + dy * dy + dz * dz);
+  }
+  dist[e] = d;
+  if (gate_w) {
+    float a = gate_b;
+    if (s >= 0) {
+      const int ty = etype[e];
+#pragma unroll 4
+      for (int j = 0; j < TD_NG; ++j) {
+        const float u = d - offsets[j];
+        a = fmaf(expf(coeff * (u * u)), gate_w[ty * TD_NG + j], a);
+      }
+    }
+    gate[e] = s >= 0 ? 1.0f / (1.0f + expf(-a)) : 0.0f;
+  }
+}
+
+void td_launch_edge_geom_rows(const float4* xm, const int* src, const unsigned char* etype, const int* rows, int n_rows, int k, float* dist,
+                              const float* gate_w, float gate_b, const float* offsets, float coeff, float* gate, cudaStream_t st) {
+  const long long n = (long long)n_rows * k;
+  if (n > 0) edge_geom_rows_kernel<<<(int)((n + 255) / 256), 256, 0, st>>>(xm, src, etype, rows, n, k, dist, gate_w, gate_b, offsets, coeff, gate);
+}
+
 // Compact the relevant-node flags into a list (order irrelevant: every row is processed independently); consumers bound by *n_rel.
 __global__ void rel_compact_kernel(const unsigned char* __restrict__ flag, int n_nodes, int* __restrict__ rel_list, int* __restrict__ n_rel) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;

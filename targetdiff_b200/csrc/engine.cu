@@ -58,6 +58,12 @@ struct DevBuf {
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
+struct TdLayer {
+  std::vector<TdSubLayer> x2h, h2x;   // num_x2h / num_h2x sub-layers, in evaluation order (reference models/uni_transformer.py:164-179)
+  const float* offsets;   // [20] gaussian centres of this layer (distance_expansion.offset)
+  float coeff;            // -0.5/(offset[1]-offset[0])^2   (reference models/common.py:17)
+};
+
 enum { EV_AGG_H = 0, EV_AGG_X = 1, EV_EDGE_MLP = 2, EV_TOTAL = 3, EV_KINDS = 4 };
 struct EvPair { cudaEvent_t a, b; int kind; };
 
@@ -76,9 +82,12 @@ struct tdiff_engine {
   float ew_b2 = 0.f, ew_coeff = -0.5f;
   // config-surface options (tdiff_config): blocks, edge-gate flavour, node_output MLP, time embedding
   int num_blocks = 1, ew_mode = 0 /* 0 global, 1 'r', 2 'm', 3 none */, out_fc = 0, time_emb = 0;
+  // layer form (tdiff_config.sublayers): x2h / h2x sub-layers per layer; sync_twoup: the h2x sub-layers read the layer's input h
+  int num_x2h = 1, num_h2x = 1, sync_twoup = 0;
   const float* w_time = nullptr;        // time_emb 'simple': the ligand embedding's extra input column
   const float* zeros128 = nullptr;
-  DevBuf ew_x2h, ew_h2x, hagg, time_norm;   // 'r' gates per slot (per layer, both sub-layers); x2h aggregate for node_output; t / T per graph
+  DevBuf ew_x2h, ew_h2x, hagg, time_norm;   // 'r' gates per slot (current x2h / h2x sub-layer); x2h aggregate for node_output; t / T per graph
+  DevBuf h_sync;                            // sync_twoup: the layer's input h, read by its h2x sub-layers
   const float *hd_w1t = nullptr, *hd_b1 = nullptr, *hd_w2 = nullptr, *hd_b2 = nullptr;
   const float *t_c0 = nullptr, *t_ct = nullptr, *t_logvar = nullptr, *t_la = nullptr, *t_l1ma = nullptr, *t_lca = nullptr, *t_l1mca = nullptr,
               *t_sra = nullptr, *t_srm1 = nullptr;
@@ -100,14 +109,15 @@ struct tdiff_engine {
   long long x2h_n_dst = 0, x2h_split = 0, lig_n_dst = 0;
   int row_pad = 4;                      // destinations per class are padded so that class boundaries fall on 128-row tile boundaries
   // Ligand-free cache (exact): protein atoms never move and their embedding is step-invariant, so a protein node that is neither
-  // touched by a ligand atom nor (transitively, layer by layer) fed by a touched node has the same features after x2h layer l in
-  // every denoising step.  Those values are computed once per bound batch (h_free[l]); per step the first `free_depth` x2h layers
-  // only visit the dirty destinations (free_rows[l]) and the clean rows are restored from the cache.
-  int free_depth = 0;                   // cached x2h layers of this batch (0 = off)
+  // touched by a ligand atom nor (transitively, x2h evaluation by evaluation) fed by a touched node has the same features after x2h
+  // sub-layer evaluation g of block 0 in every denoising step (h2x sub-layers never change h).  Those values are computed once per
+  // bound batch (h_free[g]); per step the first `free_depth` x2h evaluations only visit the dirty destinations (free_rows[g]) and the
+  // clean rows are restored from the cache.
+  int free_depth = 0;                   // cached x2h sub-layer evaluations of this batch (0 = off)
   int env_free_depth = 2;               // TDIFF_FREE_DEPTH (default 2; 0 disables)
   bool free_ready = false;
   DevBuf h_free, dirty, free_rows, free_counts, lig_save;
-  long long free_stride = 0;            // ints per layer in free_rows
+  long long free_stride = 0;            // ints per cached evaluation in free_rows
   DevBuf xm0, xm1, offset, h0, h, P, q, src, src_prev, etype, e_w, dist, kbuf, vbuf, v16, lig_pos, lig_v, logits;
   DevBuf step, err_flag, node_off, total_edges;
   DevBuf stage[8];   // staging for tdiff_sample_host
@@ -384,6 +394,14 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
     return set_err(TDIFF_EINVAL, "model_mean_type=%d (0 = C0, 1 = noise)", cfg->model_mean_type);
   for (int r : cfg->reserved)
     if (r != 0) return set_err(TDIFF_EINVAL, "tdiff_config.reserved must be 0");
+  int num_x2h = 1, num_h2x = 1, sync_twoup = 0;
+  if (cfg->sublayers != 0) {
+    const unsigned s = (unsigned)cfg->sublayers;
+    num_x2h = (int)(s & 0xffu); num_h2x = (int)((s >> 8) & 0xffu); sync_twoup = (int)((s >> 16) & 0xffu);
+    if ((s >> 24) != 1u || num_x2h > 16 || num_h2x > 16 || sync_twoup > 1)
+      return set_err(TDIFF_EINVAL, "sublayers=0x%08x: expected 0 or 1<<24 | sync_twoup<<16 | num_h2x<<8 | num_x2h with num_x2h, num_h2x in 0..16 and "
+                     "sync_twoup in 0..1", s);
+  }
   if (cfg->cutoff_mode != 0 && cfg->cutoff_mode != 1) return set_err(TDIFF_EINVAL, "cutoff_mode=%d (0 = 'knn', 1 = 'hybrid')", cfg->cutoff_mode);
   if (cfg->num_blocks < 0 || cfg->num_blocks > 16 || cfg->ew_net_type < 0 || cfg->ew_net_type > 3 || (cfg->x2h_out_fc != 0 && cfg->x2h_out_fc != 1) ||
       (cfg->time_emb != 0 && cfg->time_emb != 1))
@@ -406,6 +424,7 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
   tdiff_engine* e = new tdiff_engine();
   e->cfg = *cfg; e->device = device; e->sm_count = prop.multiProcessorCount; e->K = e->KQ = cfg->knn; e->hybrid = cfg->cutoff_mode;
   e->num_blocks = cfg->num_blocks > 1 ? cfg->num_blocks : 1; e->ew_mode = cfg->ew_net_type; e->out_fc = cfg->x2h_out_fc; e->time_emb = cfg->time_emb;
+  e->num_x2h = num_x2h; e->num_h2x = num_h2x; e->sync_twoup = sync_twoup;
   // the edge-MLP mode decides where the packer puts the LayerNorm gain's sign (pack_edge_mlp)
   if (const char* mode = getenv("TDIFF_EDGE_MLP")) {
     if (!strcmp(mode, "simt")) e->mlp_mode = 0;
@@ -478,15 +497,20 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
     memcpy(&pk.host[o_hb1], hb1, TD_H * 4); memcpy(&pk.host[o_hw2], hw2, (size_t)KC * TD_H * 4); memcpy(&pk.host[o_hb2], hb2, KC * 4);
   }
   // attention layers
-  std::vector<SubOff> sx(L), sh(L);
+  std::vector<std::vector<SubOff>> sx(L, std::vector<SubOff>(num_x2h)), sh(L, std::vector<SubOff>(num_h2x));
   std::vector<size_t> o_off(L);
   std::vector<float> coeffs(L, -0.5f);
   for (int l = 0; l < L; ++l) {
     const std::string p = "refine_net.base_block." + std::to_string(l);
-    if (!pack_sublayer(pk, p + ".x2h_layers.0", "hk_func", "hv_func", "hq_func", TD_H, v4, sx[l])) break;
-    if (!pack_sublayer(pk, p + ".h2x_layers.0", "xk_func", "xv_func", "xq_func", TD_HEADS, v4, sh[l])) break;
-    if (!pack_sublayer_options(pk, p + ".x2h_layers.0", cfg->ew_net_type == 1 ? 4 * TD_NG : cfg->ew_net_type == 2 ? TD_H : 0, cfg->x2h_out_fc != 0, sx[l])) break;
-    if (!pack_sublayer_options(pk, p + ".h2x_layers.0", cfg->ew_net_type == 1 ? 4 * TD_NG : 0, false, sh[l])) break;
+    bool ok = true;
+    for (int i = 0; ok && i < num_x2h; ++i) ok = pack_sublayer(pk, p + ".x2h_layers." + std::to_string(i), "hk_func", "hv_func", "hq_func", TD_H, v4, sx[l][i]);
+    for (int i = 0; ok && i < num_h2x; ++i) ok = pack_sublayer(pk, p + ".h2x_layers." + std::to_string(i), "xk_func", "xv_func", "xq_func", TD_HEADS, v4, sh[l][i]);
+    for (int i = 0; ok && i < num_x2h; ++i)
+      ok = pack_sublayer_options(pk, p + ".x2h_layers." + std::to_string(i), cfg->ew_net_type == 1 ? 4 * TD_NG : cfg->ew_net_type == 2 ? TD_H : 0,
+                                 cfg->x2h_out_fc != 0, sx[l][i]);
+    for (int i = 0; ok && i < num_h2x; ++i)
+      ok = pack_sublayer_options(pk, p + ".h2x_layers." + std::to_string(i), cfg->ew_net_type == 1 ? 4 * TD_NG : 0, false, sh[l][i]);
+    if (!ok) break;
     const float* off = pk.get(p + ".distance_expansion.offset", TD_NG);
     o_off[l] = pk.alloc(TD_NG);
     if (off) {
@@ -514,6 +538,10 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
     cudaFree(e->arena); cudaFree(e->img_arena); delete e;
     return set_err(TDIFF_EINVAL, "ew_net_type != 'global', x2h_out_fc and cutoff_mode 'hybrid' are implemented (and tested) in the default engine mode only (unset TDIFF_EDGE_MLP)");
   }
+  if (cfg->sublayers != 0 && !(num_x2h == 1 && num_h2x == 1 && !sync_twoup) && !(e->mlp_mode == 2 && e->mlp_v4)) {
+    cudaFree(e->arena); cudaFree(e->img_arena); delete e;
+    return set_err(TDIFF_EINVAL, "num_x2h / num_h2x != 1 and sync_twoup are implemented (and tested) in the default engine mode only (unset TDIFF_EDGE_MLP)");
+  }
   e->env_no_fused_agg = getenv("TDIFF_NO_FUSED_AGG") != nullptr;
   e->env_no_restrict = getenv("TDIFF_NO_RESTRICT") != nullptr;
   e->env_no_graph = getenv("TDIFF_NO_GRAPH") != nullptr;
@@ -534,13 +562,13 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
   for (int l = 0; l < L; ++l) {
     TdLayer& ly = e->layers[l];
     ly.offsets = A + o_off[l]; ly.coeff = coeffs[l];
-    ly.x2h.wn_t = A + sx[l].wn_t; ly.x2h.bn = A + sx[l].bn; ly.x2h.wn_img = IM ? IM + sx[l].wn_img : nullptr;
-    ly.x2h.k = mk_mlp(A, IM, sx[l].k, 0, 256); ly.x2h.v = mk_mlp(A, IM, sx[l].v, 128, 384); ly.x2h.q = mk_mlp(A, IM, sx[l].q, 512, 512);
-    ly.h2x.wn_t = A + sh[l].wn_t; ly.h2x.bn = A + sh[l].bn; ly.h2x.wn_img = IM ? IM + sh[l].wn_img : nullptr;
-    ly.h2x.k = mk_mlp(A, IM, sh[l].k, 0, 256); ly.h2x.v = mk_mlp(A, IM, sh[l].v, 128, 384); ly.h2x.q = mk_mlp(A, IM, sh[l].q, 512, 512);
-    for (int sub = 0; sub < 2; ++sub) {
-      TdSubLayer& sl = sub ? ly.h2x : ly.x2h;
-      const SubOff& so = sub ? sh[l] : sx[l];
+    ly.x2h.resize(num_x2h); ly.h2x.resize(num_h2x);
+    for (int idx = 0; idx < num_x2h + num_h2x; ++idx) {
+      const bool is_h2x = idx >= num_x2h;
+      TdSubLayer& sl = is_h2x ? ly.h2x[idx - num_x2h] : ly.x2h[idx];
+      const SubOff& so = is_h2x ? sh[l][idx - num_x2h] : sx[l][idx];
+      sl.wn_t = A + so.wn_t; sl.bn = A + so.bn; sl.wn_img = IM ? IM + so.wn_img : nullptr;
+      sl.k = mk_mlp(A, IM, so.k, 0, 256); sl.v = mk_mlp(A, IM, so.v, 128, 384); sl.q = mk_mlp(A, IM, so.q, 512, 512);
       sl.ew_w = so.ew_w >= 0 ? A + so.ew_w : nullptr; sl.ew_b = so.ew_b;
       sl.out_wa_img = so.out_wa >= 0 ? IM + so.out_wa : nullptr; sl.out_wb_img = so.out_wb >= 0 ? IM + so.out_wb : nullptr;
       sl.out_b1 = so.out_b1 >= 0 ? A + so.out_b1 : nullptr;
@@ -571,7 +599,7 @@ extern "C" void tdiff_destroy(tdiff_engine* e) {
   if (e->ev_fork) cudaEventDestroy(e->ev_fork);
   if (e->ev_join) cudaEventDestroy(e->ev_join);
   DevBuf* bufs[] = {&e->node_ptr, &e->prot_ptr, &e->prot_node, &e->prot_graph, &e->lig_node, &e->lig_graph, &e->node_lig, &e->xm0, &e->xm1,
-                    &e->rel_flag, &e->rel_list, &e->n_rel, &e->work_list, &e->n_work, &e->knn_cache, &e->x2h_rows, &e->lig_rows, &e->rel_rows, &e->rel_counts, &e->ew_x2h, &e->ew_h2x, &e->hagg, &e->time_norm, &e->h_free, &e->dirty, &e->free_rows, &e->free_counts, &e->lig_save, &e->offset, &e->h0, &e->h, &e->P, &e->q, &e->src, &e->src_prev, &e->etype, &e->e_w, &e->dist, &e->kbuf, &e->vbuf, &e->v16, &e->lig_pos,
+                    &e->rel_flag, &e->rel_list, &e->n_rel, &e->work_list, &e->n_work, &e->knn_cache, &e->x2h_rows, &e->lig_rows, &e->rel_rows, &e->rel_counts, &e->ew_x2h, &e->ew_h2x, &e->h_sync, &e->hagg, &e->time_norm, &e->h_free, &e->dirty, &e->free_rows, &e->free_counts, &e->lig_save, &e->offset, &e->h0, &e->h, &e->P, &e->q, &e->src, &e->src_prev, &e->etype, &e->e_w, &e->dist, &e->kbuf, &e->vbuf, &e->v16, &e->lig_pos,
                     &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges};
   for (auto* b : bufs) b->release();
   for (auto& b : e->stage) b.release();
@@ -648,6 +676,7 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   const bool fuse = v4 && K == 32 && !e->env_no_fused_agg && e->ew_mode != 2;      // 'm' gates need the value rows (unfused aggregation)
   if (e->ew_mode == 1) bad |= e->ew_x2h.ensure(slots * 4) | e->ew_h2x.ensure(slots * 4);
   if (e->out_fc) bad |= e->hagg.ensure((size_t)N * TD_H * 4);
+  if (e->sync_twoup && e->num_x2h > 0 && e->num_h2x > 0) bad |= e->h_sync.ensure((size_t)N * TD_H * 4);
   if (e->time_emb) bad |= e->time_norm.ensure((size_t)B * 4 + 16);
   bad |= e->kbuf.ensure(v4 ? (size_t)(nPpad + nLpad) * K * TD_HEADS * 4 + 64 : slots * TD_H * 4);
   if (!fuse) bad |= e->vbuf.ensure(slots * TD_H * 4);
@@ -658,7 +687,9 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   for (int g = 0; g < B; ++g) if (pc[g] < min_pc) min_pc = pc[g];
   e->free_ready = false;
   e->free_depth = (fuse && !e->hybrid && Nl > 0 && min_pc > K) ? e->env_free_depth : 0;      // (only block 0 of a multi-block network uses it)
-  if (e->free_depth > (int)e->layers.size() - 1) e->free_depth = (int)e->layers.size() - 1;
+  // counted in x2h sub-layer evaluations of block 0; the last one may be restricted to the relevant nodes and is never cached
+  const int x2h_evals = (int)e->layers.size() * e->num_x2h;
+  if (e->free_depth > x2h_evals - 1) e->free_depth = x2h_evals - 1 > 0 ? x2h_evals - 1 : 0;
   if (e->free_depth > 0)
     bad |= e->h_free.ensure((size_t)e->free_depth * N * TD_H * 4) | e->dirty.ensure((size_t)e->free_depth * N + 16) |
            e->free_rows.ensure((size_t)e->free_depth * x2h_rows.size() * 4 + 4) | e->free_counts.ensure((size_t)e->free_depth * 16) |
@@ -810,8 +841,10 @@ void node_side(tdiff_engine* e, const float* h, int N, const TdSubLayer& sl, flo
 }
 
 // One evaluation of the network on the bound batch (reference ScorePosNet3D.forward -> UniTransformerO2TwoUpdateGeneral.forward)
-// `free_build` > 0: ligand-free cache construction -- only the first `free_build` x2h layers, features saved after each (ligand parked far away)
-void run_forward(tdiff_engine* e, cudaStream_t st, int fix_x, int free_build = 0) {
+// `free_build` > 0: ligand-free cache construction -- only the first `free_build` x2h sub-layer evaluations, features saved after each
+// (ligand parked far away).  `blk_pos` [(B+1),Nl,3] / `blk_logits` [(B+1),Nl,K] (optional, tdiff_forward_blocks): ligand coordinates and
+// type logits before block 0 and after every block (reference return_all, models/uni_transformer.py:303-327)
+void run_forward(tdiff_engine* e, cudaStream_t st, int fix_x, int free_build = 0, float* blk_pos = nullptr, float* blk_logits = nullptr) {
   const int N = e->N, Nl = e->Nl, K = e->K;
   float4* xm[2] = {e->xm0.as<float4>(), e->xm1.as<float4>()};
   const int* src = e->src.as<int>();
@@ -824,6 +857,18 @@ void run_forward(tdiff_engine* e, cudaStream_t st, int fix_x, int free_build = 0
                    e->lig_graph.as<int>(), N, h, st);
   e->launches += 2;
   int cur = 0;
+  const int KC = e->cfg.num_classes;
+  auto snapshot = [&](int i) {
+    if (blk_pos) {
+      td_launch_gather_xyz(xm[cur], e->lig_node.as<int>(), Nl, blk_pos + (size_t)i * Nl * 3, st);
+      e->launches += 1;
+    }
+    if (blk_logits) {
+      td_launch_head(h, e->lig_node.as<int>(), Nl, e->hd_w1t, e->hd_b1, e->hd_w2, e->hd_b2, KC, blk_logits + (size_t)i * Nl * KC, st);
+      e->launches += 1;
+    }
+  };
+  if (Nl > 0) snapshot(0);
   const int n_blocks = free_build ? 1 : e->num_blocks;
   for (int blk = 0; blk < n_blocks; ++blk) {
     // ---- graph of this block from the current coordinates (reference models/uni_transformer.py:306-318)
@@ -847,95 +892,121 @@ void run_forward(tdiff_engine* e, cudaStream_t st, int fix_x, int free_build = 0
     }
     td_launch_rel_compact(e->rel_flag.as<unsigned char>(), N, e->rel_list.as<int>(), e->n_rel.as<int>(), st);
     e->launches += 4;
-    if (fused_logits(e) && e->restrict_last && last_blk) {       // class-sorted list of the relevant destinations for the last x2h
+    if (fused_logits(e) && e->restrict_last && last_blk && e->num_x2h > 0) {   // class-sorted list of the relevant destinations for the last x2h
       td_launch_rel_rows(e->rel_flag.as<unsigned char>(), xm[cur], N, e->lig_rows.as<int>(), (int)e->lig_n_dst, e->row_pad, e->rel_rows.as<int>(),
                          e->rel_counts.as<int>(), st);
       e->launches += 2;
     }
     const float4* xm_blk = xm[cur];                  // coordinates the block's graph was built from (protein flags for the cache kernels)
-    const size_t n_layers = free_build ? (size_t)free_build : e->layers.size();
-    for (size_t l = 0; l < n_layers; ++l) {
+    const int NX = e->num_x2h, NH = e->num_h2x;
+    const size_t L = e->layers.size();
+    int g = 0;                                       // x2h sub-layer evaluations of this block so far (the ligand-free cache's unit)
+    for (size_t l = 0; l < L && !(free_build && g >= free_build); ++l) {
       const TdLayer& ly = e->layers[l];
-      const int fl = (int)l < use_free ? (int)l : -1;
-      // per-sub-layer edge gates: the global gate, or the layer's own 'r' gates (evaluated with the edge lengths), or 1
+      // per-sub-layer edge gates: the global gate, or the current sub-layer's own 'r' gates (evaluated with the edge lengths), or 1
       const float* ew_x = e->ew_mode == 1 ? e->ew_x2h.as<float>() : e->e_w.as<float>();
       const float* ew_h = e->ew_mode == 1 ? e->ew_h2x.as<float>() : e->e_w.as<float>();
-      // ---- x2h: h <- h + sum_e alpha * v * e_w   (+ node_output MLP with x2h_out_fc)
-      node_side(e, h, N, ly.x2h, P, q, st);
-      if (e->mlp_mode != 0) {
-        TdEwR ew = {nullptr, nullptr, 0.f, 0.f, ly.offsets, ly.coeff, nullptr, nullptr};
-        if (e->ew_mode == 1) { ew.w_x2h = ly.x2h.ew_w; ew.w_h2x = ly.h2x.ew_w; ew.b_x2h = ly.x2h.ew_b; ew.b_h2x = ly.h2x.ew_b; ew.out_x2h = e->ew_x2h.as<float>(); ew.out_h2x = e->ew_h2x.as<float>(); }
-        td_launch_edge_geom(xm[cur], src, etype, N, K, e->dist.as<float>(), ew, st);
-        e->launches += 1;
+      // h2x only moves ligand atoms; with fix_x its result is discarded (models/uni_transformer.py:204-206)
+      const bool run_h2x = !free_build && !fix_x && Nl > 0 && NH > 0;
+      // sync_twoup: the h2x sub-layers read the layer's input h (:199); the x2h launches update h in place, so keep a copy
+      const float* h_h2x = h;
+      if (e->sync_twoup && run_h2x && NX > 0) {
+        cudaMemcpyAsync(e->h_sync.p, h, (size_t)N * TD_H * 4, cudaMemcpyDeviceToDevice, st);
+        h_h2x = e->h_sync.as<float>();
       }
-      // k == 32: a 128-row tile is 4 complete destinations -> the value launch also performs the softmax aggregation (h += ...)
-      const bool fuse_agg = fused_logits(e) && K == 32 && !e->env_no_fused_agg && e->ew_mode != 2;
-      // sampling loop, last layer: only the ligand atoms' features feed the type head and only ligand atoms + their neighbours feed
-      // the last h2x, so x2h is evaluated for those destinations only (device-compacted list; final_h of other nodes is not produced)
-      const bool sub = fuse_agg && e->restrict_last && last_blk && l + 1 == e->layers.size() && !e->env_no_restrict && !e->out_fc;
-      const RowList rl = sub ? ROWS_RELEVANT : ROWS_ALL;
-      float* agg_target = h;
-      if (e->out_fc) {               // node_output needs the bare aggregate: accumulate into a zeroed buffer instead of h
-        agg_target = e->hagg.as<float>();
-        cudaMemsetAsync(agg_target, 0, (size_t)N * TD_H * 4, st);
+      for (int i = 0; i < NX && !(free_build && g >= free_build); ++i, ++g) {
+        const TdSubLayer& sx = ly.x2h[i];
+        const int fl = g < use_free ? g : -1;
+        // ---- x2h: h <- h + sum_e alpha * v * e_w   (+ node_output MLP with x2h_out_fc)
+        node_side(e, h, N, sx, P, q, st);
+        // edge lengths from the layer's input coordinates (x does not move during x2h); 'r': this x2h sub-layer's gates and the first
+        // h2x sub-layer's (with no h2x sub-layer, a throw-away second set)
+        if (e->mlp_mode != 0 && (i == 0 || e->ew_mode == 1)) {
+          TdEwR ew = {nullptr, nullptr, 0.f, 0.f, ly.offsets, ly.coeff, nullptr, nullptr};
+          if (e->ew_mode == 1) {
+            const TdSubLayer& sh0 = NH > 0 ? ly.h2x[0] : sx;
+            ew.w_x2h = sx.ew_w; ew.w_h2x = sh0.ew_w; ew.b_x2h = sx.ew_b; ew.b_h2x = sh0.ew_b; ew.out_x2h = e->ew_x2h.as<float>(); ew.out_h2x = e->ew_h2x.as<float>();
+          }
+          td_launch_edge_geom(xm[cur], src, etype, N, K, e->dist.as<float>(), ew, st);
+          e->launches += 1;
+        }
+        // k == 32: a 128-row tile is 4 complete destinations -> the value launch also performs the softmax aggregation (h += ...)
+        const bool fuse_agg = fused_logits(e) && K == 32 && !e->env_no_fused_agg && e->ew_mode != 2;
+        // sampling loop, last x2h sub-layer of the network: only the ligand atoms' features feed the type head and only ligand atoms +
+        // their neighbours feed the h2x sub-layers, so x2h is evaluated for those destinations only (device-compacted list; final_h of
+        // other nodes is not produced).  With sync_twoup the h2x sub-layers read the layer's input h, and the head the ligand rows.
+        const bool sub = fuse_agg && e->restrict_last && last_blk && l + 1 == L && i + 1 == NX && !e->env_no_restrict && !e->out_fc;
+        const RowList rl = sub ? ROWS_RELEVANT : ROWS_ALL;
+        float* agg_target = h;
+        if (e->out_fc) {               // node_output needs the bare aggregate: accumulate into a zeroed buffer instead of h
+          agg_target = e->hagg.as<float>();
+          cudaMemsetAsync(agg_target, 0, (size_t)N * TD_H * 4, st);
+        }
+        {
+          Prof pr(e, st, EV_EDGE_MLP);
+          edge_mlp(e, P, xm[cur], src, etype, rl, K, sx.k, ly.offsets, ly.coeff, e->kbuf.as<float>(), st, ew_x, fused_logits(e) ? q : nullptr, nullptr,
+                   nullptr, fuse_agg ? 1 : 0, fl);
+          edge_mlp(e, P, xm[cur], src, etype, rl, K, sx.v, ly.offsets, ly.coeff, e->vbuf.as<float>(), st, ew_x, nullptr,
+                   fuse_agg ? e->kbuf.as<float>() : nullptr, fuse_agg ? agg_target : nullptr, 0, fl);
+        }
+        if (!fuse_agg) {
+          Prof pr(e, st, EV_AGG_H);
+          if (fused_logits(e))
+            td_launch_aggregate_h_logits(e->kbuf.as<float>(), e->vbuf.as<float>(), ew_x, src, e->out_fc ? agg_target : h, agg_target, N, K,
+                                         e->ew_mode == 2 ? sx.ew_w : nullptr, sx.ew_b, st);
+          else td_launch_aggregate_h(e->kbuf.as<float>(), e->vbuf.as<float>(), e->e_w.as<float>(), src, q, h, h, N, K, st);
+        }
+        e->launches += fuse_agg ? 4 : 5;
+        if (e->out_fc) {               // h <- h + node_output([aggregate | h])   (reference models/uni_transformer.py:80-83); P is free here
+          float* t1 = P;
+          float* t2 = P + (size_t)N * TD_H;
+          TdMlp m1 = sx.out;
+          m1.b2 = e->zeros128;
+          td_launch_rows_tc(1, agg_target, TD_H, 0, N, m1, sx.out_wa_img, e->mlp_mode, t1, TD_H, 1, nullptr, nullptr, e->sm_count, st);
+          m1.b2 = sx.out_b1;
+          td_launch_rows_tc(1, h, TD_H, 0, N, m1, sx.out_wb_img, e->mlp_mode, t2, TD_H, 1, nullptr, nullptr, e->sm_count, st);
+          td_launch_add_rows(t1, t2, t1, (long long)N * TD_H, st);
+          td_launch_rows_tc(2, t1, TD_H, 0, N, sx.out, sx.out.w2_img, e->mlp_mode, t2, TD_H, 1, nullptr, nullptr, e->sm_count, st);
+          td_launch_add_rows(h, t2, h, (long long)N * TD_H, st);
+          e->launches += 6;
+        }
+        if (fl >= 0) {                 // clean protein rows: cached ligand-free features of this evaluation
+          td_launch_restore_clean(e->dirty.as<unsigned char>() + (size_t)fl * N, xm_blk, e->h_free.as<float>() + (size_t)fl * N * TD_H, N, h, st);
+          e->launches += 1;
+        }
+        if (free_build) cudaMemcpyAsync(e->h_free.as<float>() + (size_t)g * N * TD_H, h, (size_t)N * TD_H * 4, cudaMemcpyDeviceToDevice, st);
       }
-      {
-        Prof pr(e, st, EV_EDGE_MLP);
-        edge_mlp(e, P, xm[cur], src, etype, rl, K, ly.x2h.k, ly.offsets, ly.coeff, e->kbuf.as<float>(), st, ew_x, fused_logits(e) ? q : nullptr, nullptr,
-                 nullptr, fuse_agg ? 1 : 0, fl);
-        edge_mlp(e, P, xm[cur], src, etype, rl, K, ly.x2h.v, ly.offsets, ly.coeff, e->vbuf.as<float>(), st, ew_x, nullptr,
-                 fuse_agg ? e->kbuf.as<float>() : nullptr, fuse_agg ? agg_target : nullptr, 0, fl);
+      if (!run_h2x) continue;
+      // ---- h2x sub-layers: x_lig <- x_lig + mean_heads sum_e alpha * v * e_w * (x_dst - x_src), destinations = ligand atoms only; each
+      // reads the same h, and rel_x / dist are recomputed from the moved coordinates after each (models/uni_transformer.py:199-208)
+      for (int j = 0; j < NH; ++j) {
+        const TdSubLayer& sh = ly.h2x[j];
+        if (j > 0 || NX == 0) {        // edge lengths of the ligand-destination slots (the only ones an h2x reads) + this sub-layer's 'r' gates
+          td_launch_edge_geom_rows(xm[cur], src, etype, e->lig_node.as<int>(), Nl, K, e->dist.as<float>(), e->ew_mode == 1 ? sh.ew_w : nullptr, sh.ew_b,
+                                   ly.offsets, ly.coeff, e->ew_h2x.as<float>(), st);
+          e->launches += 1;
+        }
+        {
+          const bool rel = fused_logits(e) && !e->env_no_restrict;      // h2x only reads P / q of ligand atoms and their neighbours
+          node_side(e, h_h2x, N, sh, P, q, st, rel ? e->rel_list.as<int>() : nullptr, rel ? e->n_rel.as<int>() : nullptr);
+        }
+        {
+          Prof pr(e, st, EV_EDGE_MLP);
+          edge_mlp(e, P, xm[cur], src, etype, ROWS_LIGAND, K, sh.k, ly.offsets, ly.coeff, e->kbuf.as<float>(), st, ew_h, fused_logits(e) ? q : nullptr);
+          edge_mlp(e, P, xm[cur], src, etype, ROWS_LIGAND, K, sh.v, ly.offsets, ly.coeff, e->v16.as<float>(), st, ew_h);
+        }
+        {
+          Prof pr(e, st, EV_AGG_X);
+          if (fused_logits(e))
+            td_launch_aggregate_x_logits(e->kbuf.as<float>(), e->v16.as<float>(), ew_h, src, xm[cur], e->lig_node.as<int>(), xm[cur ^ 1], Nl, K, st);
+          else
+            td_launch_aggregate_x(e->kbuf.as<float>(), e->v16.as<float>(), e->e_w.as<float>(), src, q, xm[cur], e->lig_node.as<int>(), xm[cur ^ 1], Nl, K, st);
+        }
+        e->launches += 5;
+        cur ^= 1;
       }
-      if (!fuse_agg) {
-        Prof pr(e, st, EV_AGG_H);
-        if (fused_logits(e))
-          td_launch_aggregate_h_logits(e->kbuf.as<float>(), e->vbuf.as<float>(), ew_x, src, e->out_fc ? agg_target : h, agg_target, N, K,
-                                       e->ew_mode == 2 ? ly.x2h.ew_w : nullptr, ly.x2h.ew_b, st);
-        else td_launch_aggregate_h(e->kbuf.as<float>(), e->vbuf.as<float>(), e->e_w.as<float>(), src, q, h, h, N, K, st);
-      }
-      e->launches += fuse_agg ? 4 : 5;
-      if (e->out_fc) {               // h <- h + node_output([aggregate | h])   (reference models/uni_transformer.py:80-83); P is free here
-        float* t1 = P;
-        float* t2 = P + (size_t)N * TD_H;
-        TdMlp m1 = ly.x2h.out;
-        m1.b2 = e->zeros128;
-        td_launch_rows_tc(1, agg_target, TD_H, 0, N, m1, ly.x2h.out_wa_img, e->mlp_mode, t1, TD_H, 1, nullptr, nullptr, e->sm_count, st);
-        m1.b2 = ly.x2h.out_b1;
-        td_launch_rows_tc(1, h, TD_H, 0, N, m1, ly.x2h.out_wb_img, e->mlp_mode, t2, TD_H, 1, nullptr, nullptr, e->sm_count, st);
-        td_launch_add_rows(t1, t2, t1, (long long)N * TD_H, st);
-        td_launch_rows_tc(2, t1, TD_H, 0, N, ly.x2h.out, ly.x2h.out.w2_img, e->mlp_mode, t2, TD_H, 1, nullptr, nullptr, e->sm_count, st);
-        td_launch_add_rows(h, t2, h, (long long)N * TD_H, st);
-        e->launches += 6;
-      }
-      if (fl >= 0) {                 // clean protein rows: cached ligand-free features of this layer
-        td_launch_restore_clean(e->dirty.as<unsigned char>() + (size_t)fl * N, xm_blk, e->h_free.as<float>() + (size_t)fl * N * TD_H, N, h, st);
-        e->launches += 1;
-      }
-      if (free_build) {
-        cudaMemcpyAsync(e->h_free.as<float>() + l * (size_t)N * TD_H, h, (size_t)N * TD_H * 4, cudaMemcpyDeviceToDevice, st);
-        continue;
-      }
-      if (fix_x || Nl == 0) continue;     // h2x only moves ligand atoms; with fix_x its result is discarded (:204-206)
-      // ---- h2x: x_lig <- x_lig + mean_heads sum_e alpha * v * e_w * (x_dst - x_src), destinations = ligand atoms only
-      {
-        const bool rel = fused_logits(e) && !e->env_no_restrict;      // h2x only reads P / q of ligand atoms and their neighbours
-        node_side(e, h, N, ly.h2x, P, q, st, rel ? e->rel_list.as<int>() : nullptr, rel ? e->n_rel.as<int>() : nullptr);
-      }
-      {
-        Prof pr(e, st, EV_EDGE_MLP);
-        edge_mlp(e, P, xm[cur], src, etype, ROWS_LIGAND, K, ly.h2x.k, ly.offsets, ly.coeff, e->kbuf.as<float>(), st, ew_h, fused_logits(e) ? q : nullptr);
-        edge_mlp(e, P, xm[cur], src, etype, ROWS_LIGAND, K, ly.h2x.v, ly.offsets, ly.coeff, e->v16.as<float>(), st, ew_h);
-      }
-      {
-        Prof pr(e, st, EV_AGG_X);
-        if (fused_logits(e))
-          td_launch_aggregate_x_logits(e->kbuf.as<float>(), e->v16.as<float>(), ew_h, src, xm[cur], e->lig_node.as<int>(), xm[cur ^ 1], Nl, K, st);
-        else
-          td_launch_aggregate_x(e->kbuf.as<float>(), e->v16.as<float>(), e->e_w.as<float>(), src, q, xm[cur], e->lig_node.as<int>(), xm[cur ^ 1], Nl, K, st);
-      }
-      e->launches += 5;
-      cur ^= 1;
     }
+    if (Nl > 0) snapshot(blk + 1);
   }
   if (free_build) return;
   td_launch_head(h, e->lig_node.as<int>(), Nl, e->hd_w1t, e->hd_b1, e->hd_w2, e->hd_b2, e->cfg.num_classes, e->logits.as<float>(), st);
@@ -955,12 +1026,14 @@ extern "C" int tdiff_set_time(tdiff_engine* e, const float* d_time_norm, void* s
   return TDIFF_OK;
 }
 
-extern "C" int tdiff_forward(tdiff_engine* e, float* d_pred_pos, float* d_pred_logits, float* d_final_h, int fix_x, void* stream) {
+namespace {
+int forward_impl(tdiff_engine* e, float* d_pred_pos, float* d_pred_logits, float* d_final_h, int fix_x, float* d_block_pos, float* d_block_logits,
+                 void* stream) {
   if (!e || !e->bound || !e->has_ligand) return set_err(TDIFF_ESTATE, "forward needs bind_batch + set_ligand first");
   cudaStream_t st = (cudaStream_t)stream;
   CK(cudaSetDevice(e->device));
   Prof* total = new Prof(e, st, EV_TOTAL);
-  run_forward(e, st, fix_x);
+  run_forward(e, st, fix_x, 0, d_block_pos, d_block_logits);
   delete total;
   const float4* xf = e->final_buf ? e->xm1.as<float4>() : e->xm0.as<float4>();
   if (d_pred_pos) { td_launch_gather_xyz(xf, e->lig_node.as<int>(), e->Nl, d_pred_pos, st); e->launches += 1; }
@@ -968,6 +1041,16 @@ extern "C" int tdiff_forward(tdiff_engine* e, float* d_pred_pos, float* d_pred_l
   if (d_final_h) CK(cudaMemcpyAsync(d_final_h, e->h.p, (size_t)e->N * TD_H * 4, cudaMemcpyDeviceToDevice, st));
   CK(cudaGetLastError());
   return TDIFF_OK;
+}
+}  // namespace
+
+extern "C" int tdiff_forward(tdiff_engine* e, float* d_pred_pos, float* d_pred_logits, float* d_final_h, int fix_x, void* stream) {
+  return forward_impl(e, d_pred_pos, d_pred_logits, d_final_h, fix_x, nullptr, nullptr, stream);
+}
+
+extern "C" int tdiff_forward_blocks(tdiff_engine* e, float* d_pred_pos, float* d_pred_logits, float* d_final_h, int fix_x, float* d_block_pos,
+                                    float* d_block_logits, void* stream) {
+  return forward_impl(e, d_pred_pos, d_pred_logits, d_final_h, fix_x, d_block_pos, d_block_logits, stream);
 }
 
 extern "C" int64_t tdiff_num_edges(tdiff_engine* e, void* stream) {

@@ -60,12 +60,6 @@ struct TdSubLayer {       // x2h or h2x
   TdMlp out;                         // LayerNorm affine + second Linear (ln_g, ln_b, b2, w2_img)
 };
 
-struct TdLayer {
-  TdSubLayer x2h, h2x;
-  const float* offsets;   // [20] gaussian centres of this layer (distance_expansion.offset)
-  float coeff;            // -0.5/(offset[1]-offset[0])^2   (reference models/common.py:17)
-};
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -167,6 +161,8 @@ void td_launch_node_q(const float* P, int n_nodes, TdMlp q, float* qout, cudaStr
 void td_launch_edge_mlp(const float* P, const float4* xm, const int* src, const unsigned char* etype, const int* row_nodes,
                         long long n_rows, int k, TdMlp m, const float* offsets, float coeff, float* out, int sm_count, cudaStream_t st);
 void td_launch_edge_geom(const float4* xm, const int* src, const unsigned char* etype, int n_nodes, int k, float* dist, const TdEwR& ew, cudaStream_t st);
+void td_launch_edge_geom_rows(const float4* xm, const int* src, const unsigned char* etype, const int* rows, int n_rows, int k, float* dist,
+                              const float* gate_w, float gate_b, const float* offsets, float coeff, float* gate, cudaStream_t st);
 void td_launch_add_rows(const float* a, const float* b, float* out, long long n_floats, cudaStream_t st);
 void td_launch_set_time(const int* step, int t_start, int n_timesteps, int n_graphs, float* time_norm, cudaStream_t st);
 void td_launch_edge_mlp_tc(const float* P, const float4* xm, const int* src, const unsigned char* etype, const float* dist,

@@ -161,6 +161,14 @@ def log_sample_categorical(logits):
     return (gumbel + logits).argmax(dim=-1)
 
 
+def sublayer_code(cfg):
+    """`tdiff_config.sublayers` for the layer form (num_x2h, num_h2x, sync_twoup): 0 for the reference default (1, 1, False)."""
+    nx, nh, sync = int(cfg.get('num_x2h', 1)), int(cfg.get('num_h2x', 1)), int(bool(cfg.get('sync_twoup', False)))
+    if (nx, nh, sync) == (1, 1, 0):
+        return 0
+    return 1 << 24 | sync << 16 | nh << 8 | nx
+
+
 def _counts_from_batch(batch, name):
     """Per-graph atom counts from a sorted PyG-style batch vector (host list)."""
     if batch.numel() == 0:
@@ -251,7 +259,8 @@ class ScorePosNet3D(nn.Module):
                                 self.num_classes, self.protein_atom_feature_dim, self.num_timesteps,
                                 {'C0': 0, 'noise': 1}[self.model_mean_type], int(self.config.num_blocks),
                                 {'global': 0, 'r': 1, 'm': 2, 'none': 3}[self.config.ew_net_type], int(bool(self.config.x2h_out_fc)),
-                                1 if self.time_emb_dim > 0 else 0, {'knn': 0, 'hybrid': 1}[self.config.get('cutoff_mode', 'knn')])
+                                1 if self.time_emb_dim > 0 else 0, {'knn': 0, 'hybrid': 1}[self.config.get('cutoff_mode', 'knn')],
+                                sublayer_code(self.config))
         out = ctypes.c_void_p()
         _lib.check(lib.tdiff_create(ctypes.byref(cfg), entries, len(sd), index, ctypes.byref(out)))
         self._engine, self._engine_device, self._bound_key = out, index, None
@@ -284,9 +293,9 @@ class ScorePosNet3D(nn.Module):
                 time_step=None, return_all=False, fix_x=False, return_edge_weight=False):
         """One network evaluation (reference models/molopt_score_model.py:313-368; `time_step` [B] is only read with time_emb_dim > 0).
         Returns {'pred_ligand_pos','pred_ligand_v','final_h','final_ligand_h'}; additionally 'edge_index' (int64 [2,E]) and, with
-        `return_edge_weight`, 'edge_weight' [E]: the global edge gate e_w in edge_index order (models/uni_transformer.py:312-316)."""
-        if return_all:
-            raise NotImplementedError('return_all=True (per-block outputs) is not implemented by the H100 engine')
+        `return_edge_weight`, 'edge_weight' [E]: the global edge gate e_w in edge_index order (models/uni_transformer.py:312-316).
+        `return_all` adds the reference's per-block lists (:360-367) of num_blocks + 1 tensors each: 'layer_pred_ligand_pos' (ligand
+        coordinates before block 0 and after every block) and 'layer_pred_ligand_v' (the type head on the ligand features there)."""
         dev = protein_pos.device
         eng = self.engine(dev)
         lib = _lib.load()
@@ -311,7 +320,14 @@ class ScorePosNet3D(nn.Module):
         pred_pos = torch.empty(Nl, 3, device=dev)
         logits = torch.empty(Nl, self.num_classes, device=dev)
         final_h = torch.empty(Np + Nl, self.hidden_dim, device=dev)
-        _lib.check(lib.tdiff_forward(eng, _ptr(pred_pos), _ptr(logits), _ptr(final_h), int(bool(fix_x)), st))
+        if return_all:
+            nb = int(self.config.get('num_blocks', 1)) + 1
+            block_pos = torch.empty(nb, Nl, 3, device=dev)
+            block_logits = torch.empty(nb, Nl, self.num_classes, device=dev)
+            _lib.check(lib.tdiff_forward_blocks(eng, _ptr(pred_pos), _ptr(logits), _ptr(final_h), int(bool(fix_x)), _ptr(block_pos),
+                                                _ptr(block_logits), st))
+        else:
+            _lib.check(lib.tdiff_forward(eng, _ptr(pred_pos), _ptr(logits), _ptr(final_h), int(bool(fix_x)), st))
         E = lib.tdiff_num_edges(eng, st)
         if E < 0:
             _lib.check(int(E))
@@ -321,6 +337,9 @@ class ScorePosNet3D(nn.Module):
         lig_rows = self._ligand_rows(batch_protein, batch_ligand, B, dev)
         out = {'pred_ligand_pos': pred_pos, 'pred_ligand_v': logits, 'final_h': final_h, 'final_ligand_h': final_h[lig_rows],
                'edge_index': edge_index}
+        if return_all:
+            out['layer_pred_ligand_pos'] = list(block_pos.unbind(0))
+            out['layer_pred_ligand_v'] = list(block_logits.unbind(0))
         if return_edge_weight:
             e_w = torch.empty(E, device=dev)
             _lib.check(lib.tdiff_get_edge_weight(eng, _ptr(e_w), st))
