@@ -89,6 +89,37 @@ class LayerRef:
         return cls(sd, cfg, trace['edge_index'], trace['edge_type'], trace['mask_ligand'], x0=trace['all_x'][0], e_w=e_w, dtype=dtype)
 
 
+def embedding(sd, cfg, b, time_step=None, dtype=torch.float64):
+    """The composed node features before block 0 (`restate.embed` then `compose_context`) of batch `b`, in `dtype`: protein rows
+    W_p f + b_p with indicator 0, ligand rows W_l[:, v] + b_l (+ w_time t / T) with indicator 1.  Returns (h [N,128], mask_ligand)."""
+    sdd = _cast({k: v for k, v in sd.items() if k.endswith('_atom_emb.weight') or k.endswith('_atom_emb.bias') or
+                 k in ('betas', 'v_inference.2.weight')}, dtype)
+    with default_dtype(dtype):
+        h_p, h_l = restate.embed(sdd, cfg, b['protein_v'], b['init_ligand_v'], b['batch_ligand'], time_step)
+        h, _, _, mask = restate.compose_context(h_p, h_l, b['protein_pos'], b['init_ligand_pos'], b['batch_protein'], b['batch_ligand'])
+    return h, mask
+
+
+def head(sd, lig_h, dtype=torch.float64):
+    """The atom-type head (`restate.head`: Linear, softplus with the threshold-20 branch, minus the fp32 ln 2, Linear) on `lig_h`."""
+    sdd = _cast({k: v for k, v in sd.items() if k.startswith('v_inference.')}, dtype)
+    with default_dtype(dtype):
+        return restate.head(sdd, lig_h.to(dtype))
+
+
+def block(sd, cfg, h, x, mask_ligand, batch_all, dtype=torch.float64):
+    """One block of `restate.refine_net` from its input (h, x) [N,...] in the composed node order: the graph rebuilt from `x` as it
+    is (fp32 coordinates; `knn_graph_canonical` or `hybrid_graph`), the edge types, the global gate in `dtype`
+    (`global_edge_weight`), then the block's num_layers attention layers in `dtype`.  Returns (h, x, edge_index, e_w)."""
+    c = dict(DEFAULT_MODEL_CONFIG, **(cfg or {}))
+    edge_index = restate.connect_edge(x.float(), c, mask_ligand, batch_all)
+    edge_type = restate.build_edge_type(edge_index, mask_ligand).argmax(-1)
+    ref = LayerRef(sd, c, edge_index, edge_type, mask_ligand, x0=x, dtype=dtype)
+    for l in range(c['num_layers']):
+        h, x = ref(l, h, x)
+    return h, x, edge_index, ref.e_w
+
+
 def row_error(got, want, inp, rows=None):
     """Per-row error of one layer's output:  |got - want|_inf / max(|want - inp|_inf, 0.01 * median_r |want - inp|_inf),
     i.e. relative to the size of the row's update, with a floor for rows the layer barely moves.  `rows`: boolean row selection."""

@@ -351,28 +351,43 @@ def compose_context(h_protein, h_ligand, pos_protein, pos_ligand, batch_protein,
             batch_ctx[sort_idx], mask_ligand)
 
 
+def embed(sd, cfg, protein_v, ligand_v, batch_ligand, time_step=None):
+    """The protein and ligand node features before compose_context (:317-338), each with the node-indicator column; the ligand
+    input is the one-hot of `ligand_v` over K = v_inference's class count, plus time_step / T (rounded to fp32) under 'simple'.
+    Runs in the dtype of `sd` (and of torch's default dtype, for the indicator column)."""
+    cfg = dict(DEFAULT_MODEL_CONFIG, **(cfg or {}))
+    assert cfg['node_indicator'] and (cfg['time_emb_dim'] == 0 or cfg['time_emb_mode'] == 'simple')
+    T = sd['betas'].shape[0]
+    K = sd['v_inference.2.weight'].shape[0]
+    w = sd['ligand_atom_emb.weight']
+    lig_feat = F.one_hot(ligand_v, K).to(w.dtype)                                        # :317
+    if cfg['time_emb_dim'] > 0:                                                          # :319-324
+        lig_feat = torch.cat([lig_feat, (time_step / T).float().to(w.dtype)[batch_ligand].unsqueeze(-1)], -1)
+    h_p = F.linear(protein_v.to(w.dtype), sd['protein_atom_emb.weight'], sd['protein_atom_emb.bias'])  # :333
+    h_l = F.linear(lig_feat, w, sd['ligand_atom_emb.bias'])                              # :334
+    h_p = torch.cat([h_p, torch.zeros(len(h_p), 1)], -1)                                 # :336-338
+    h_l = torch.cat([h_l, torch.ones(len(h_l), 1)], -1)
+    return h_p, h_l
+
+
+def head(sd, lig_h):
+    """v_inference (:307-311,352): Linear -> ShiftedSoftplus -> Linear, in the dtype of `sd`."""
+    y = F.linear(lig_h, sd['v_inference.0.weight'], sd['v_inference.0.bias'])
+    y = F.softplus(y) - torch.log(torch.tensor(2.0, dtype=torch.float32)).item()       # common.py:156-162 (shift = fp32 log 2)
+    return F.linear(y, sd['v_inference.2.weight'], sd['v_inference.2.bias'])
+
+
 def forward(sd, cfg, protein_pos, protein_v, batch_protein, ligand_pos, ligand_v, batch_ligand,
             fix_x=False, trace=None, time_step=None):
     """ScorePosNet3D.forward, node_indicator=True (molopt_score_model.py:313-368); time_emb_dim = 0 or time_emb_mode 'simple'
     ('sin' cannot run in the reference: `time_feat` is [B, dim] but is concatenated with the [Nl, K] one-hot, :325-326)."""
     cfg = dict(DEFAULT_MODEL_CONFIG, **(cfg or {}))
-    assert cfg['node_indicator'] and (cfg['time_emb_dim'] == 0 or cfg['time_emb_mode'] == 'simple')
-    T = sd['betas'].shape[0]
-    K = sd['ligand_atom_emb.weight'].shape[1] - (1 if cfg['time_emb_dim'] > 0 else 0)
-    lig_feat = F.one_hot(ligand_v, K).float()                                            # :317
-    if cfg['time_emb_dim'] > 0:                                                          # :319-324
-        lig_feat = torch.cat([lig_feat, (time_step / T)[batch_ligand].unsqueeze(-1)], -1)
-    h_p = F.linear(protein_v, sd['protein_atom_emb.weight'], sd['protein_atom_emb.bias'])  # :333
-    h_l = F.linear(lig_feat, sd['ligand_atom_emb.weight'], sd['ligand_atom_emb.bias'])     # :334
-    h_p = torch.cat([h_p, torch.zeros(len(h_p), 1)], -1)                                 # :336-338
-    h_l = torch.cat([h_l, torch.ones(len(h_l), 1)], -1)
+    h_p, h_l = embed(sd, cfg, protein_v, ligand_v, batch_ligand, time_step)
     h_all, pos_all, batch_all, mask_ligand = compose_context(h_p, h_l, protein_pos, ligand_pos, batch_protein, batch_ligand)
     out = refine_net(sd, cfg, h_all, pos_all, mask_ligand, batch_all, fix_x=fix_x, trace=trace)   # :349
     final_pos, final_h = out['x'], out['h']
     lig_h = final_h[mask_ligand]                                                         # :350-351
-    y = F.linear(lig_h, sd['v_inference.0.weight'], sd['v_inference.0.bias'])            # :307-311,352
-    y = F.softplus(y) - torch.log(torch.tensor(2.0)).item()     # common.py:156-162 (shift = fp32 log 2)
-    logits = F.linear(y, sd['v_inference.2.weight'], sd['v_inference.2.bias'])
+    logits = head(sd, lig_h)
     if trace is not None:
         trace.update(mask_ligand=mask_ligand, batch_all=batch_all)
     return {'pred_ligand_pos': final_pos[mask_ligand], 'pred_ligand_v': logits, 'final_h': final_h,
@@ -457,7 +472,7 @@ def sample_diffusion_ligand(sd, cfg, protein_pos, protein_atom_feature, num_samp
     which are pre-drawn here in that interleaved order and handed to `sample_diffusion` as a tape.
     Returns the reference's 7-tuple (positions float64 numpy, trajectories [steps, atoms, ...]); the time list holds zeros."""
     c = dict(DEFAULT_MODEL_CONFIG, **(cfg or {}))
-    K = sd['ligand_atom_emb.weight'].shape[1]
+    K = sd['v_inference.2.weight'].shape[0]       # not ligand_atom_emb's input width: that is K + 1 with a time embedding
     T = sd['betas'].shape[0]
     S = T if num_steps is None else num_steps
     all_pos, all_v, all_pos_traj, all_v_traj, all_v0_traj, all_vt_traj, time_list = [], [], [], [], [], [], []
@@ -535,7 +550,7 @@ def likelihood_estimation(sd, cfg, protein_pos, protein_v, batch_protein, ligand
     `v_uniform` [Nl,K] (rand_like inside q_v_sample, :394-398 via :160-166)."""
     c = dict(DEFAULT_MODEL_CONFIG, **(cfg or {}))
     T = c['num_diffusion_timesteps']
-    K = sd['ligand_atom_emb.weight'].shape[1]
+    K = sd['v_inference.2.weight'].shape[0]       # not ligand_atom_emb's input width: that is K + 1 with a time embedding
     B = int(batch_protein.max()) + 1
     protein_pos, ligand_pos, _ = center_pos(protein_pos, ligand_pos, batch_protein, batch_ligand, 'protein')
     if bool((time_step == T).all()):
@@ -556,7 +571,7 @@ def likelihood_estimation(sd, cfg, protein_pos, protein_v, batch_protein, ligand
     log_v0 = index_to_log_onehot(ligand_v, K)
     vt = log_sample_categorical_from_uniform(q_v_pred(sd, log_v0, time_step, batch_ligand, K), v_uniform)   # :586
     log_vt = index_to_log_onehot(vt, K)
-    out = forward(sd, cfg, protein_pos, protein_v, batch_protein, xt, vt, batch_ligand)  # :588-597
+    out = forward(sd, cfg, protein_pos, protein_v, batch_protein, xt, vt, batch_ligand, time_step=time_step)  # :588-597
     mean_model = q_pos_posterior(sd, out['pred_ligand_pos'], xt, time_step, batch_ligand)   # :600-603
     log_recon = F.log_softmax(out['pred_ligand_v'], dim=-1)
     log_model = q_v_posterior(sd, log_recon, log_vt, time_step, batch_ligand, K)

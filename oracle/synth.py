@@ -87,13 +87,15 @@ def state_dict_spec(cfg=None, protein_dim=PROTEIN_FEATURE_DIM, ligand_dim=LIGAND
     return spec
 
 
-def make_state_dict(seed=0, cfg=None, schedules=None, gain=1.0):
+def make_state_dict(seed=0, cfg=None, schedules=None, gain=1.0, ligand_dim=LIGAND_NUM_CLASSES):
     """Deterministic weights.  Linear: U(-1/sqrt(in), 1/sqrt(in))*gain (nn.Linear's default bound);
     LayerNorm: weight 1+0.1*N(0,1), bias 0.1*N(0,1) (non-trivial affine on purpose).
-    `schedules`: dict of the 15 fp32 tables (oracle.restate.make_schedules) -- required."""
+    `schedules`: dict of the 15 fp32 tables (oracle.restate.make_schedules) -- required.
+    `ligand_dim`: the ligand class count K (8 'basic', 13 'add_aromatic', 23 'full'); the draws follow the key order, so the
+    default K = 13 gives the same weights as before the keyword existed."""
     g = torch.Generator().manual_seed(seed)
     sd = {}
-    for key, shape, kind in state_dict_spec(cfg):
+    for key, shape, kind in state_dict_spec(cfg, ligand_dim=ligand_dim):
         if kind == 'schedule':
             sd[key] = schedules[key].clone()
         elif kind == 'zeros':
@@ -143,10 +145,10 @@ def make_pocket(seed, n_protein=300, radius=None, min_sep=1.2, cavity=4.0, cente
     return torch.from_numpy(pos), torch.from_numpy(feat)
 
 
-def make_batch(seed, n_graphs, n_protein=300, n_ligand=20, distinct_pockets=None, ligand_sizes=None):
+def make_batch(seed, n_graphs, n_protein=300, n_ligand=20, distinct_pockets=None, ligand_sizes=None, num_classes=LIGAND_NUM_CLASSES):
     """Batch in the reference's calling convention (scripts/sample_diffusion.py:42-70):
     protein_pos [Np,3], protein_v [Np,27], batch_protein [Np] i64, init_ligand_pos [Nl,3],
-    init_ligand_v [Nl] i64, batch_ligand [Nl] i64.  `distinct_pockets` pockets are cycled over graphs."""
+    init_ligand_v [Nl] i64 in 0..num_classes-1, batch_ligand [Nl] i64.  `distinct_pockets` pockets are cycled over graphs."""
     distinct_pockets = distinct_pockets or n_graphs
     pockets = [make_pocket(seed * 1000 + p, n_protein) for p in range(distinct_pockets)]
     g = torch.Generator().manual_seed(seed + 17)
@@ -161,7 +163,7 @@ def make_batch(seed, n_graphs, n_protein=300, n_ligand=20, distinct_pockets=None
         ctr = pos.mean(0, keepdim=True)
         lpos.append(ctr + torch.randn(ligand_sizes[i], 3, generator=g))
     nl = sum(ligand_sizes)
-    lig_v = torch.randint(0, LIGAND_NUM_CLASSES, (nl,), generator=g)
+    lig_v = torch.randint(0, num_classes, (nl,), generator=g)
     return dict(protein_pos=torch.cat(ppos), protein_v=torch.cat(pfeat), batch_protein=torch.cat(bp),
                 init_ligand_pos=torch.cat(lpos), init_ligand_v=lig_v, batch_ligand=torch.cat(bl))
 
