@@ -827,9 +827,13 @@ void edge_mlp(tdiff_engine* e, const float* P, const float4* xm, const int* src,
 
 // node-side GEMMs: P = h . Wn^T + bn ; q = relu(LN(P[:,512:640])) . W2q^T + b2q   (tensor cores unless TDIFF_EDGE_MLP=simt)
 // `rows` / `d_n` (optional): restrict to a node subset given as a device list (+ device count); other rows of P / q are left stale
+// Default mode (v4 edge MLPs): node_side.cu computes P[:, 0:512] and q from h, q_pre stays in registers (P[:, 512:640] is not written:
+// the v4 edge MLPs do not read it).
 void node_side(tdiff_engine* e, const float* h, int N, const TdSubLayer& sl, float* P, float* q, cudaStream_t st, const int* rows = nullptr,
                const int* d_n = nullptr) {
-  if (e->mlp_mode != 0 && sl.wn_img && sl.q.w2_img) {
+  if (fused_logits(e) && sl.wn_img && sl.q.w2_img) {
+    td_launch_node_side_v4(h, N, sl.wn_img, sl.bn, sl.q, P, q, rows, d_n, e->sm_count, st);
+  } else if (e->mlp_mode != 0 && sl.wn_img && sl.q.w2_img) {
     TdMlp pm = sl.q;
     pm.b2 = sl.bn;                 // mode 1 reads the per-column-block bias through m.b2
     td_launch_rows_tc(1, h, TD_H, 0, N, pm, sl.wn_img, e->mlp_mode, P, TD_NPROJ, TD_NPROJ / TD_H, rows, d_n, e->sm_count, st);

@@ -174,6 +174,8 @@ void td_launch_edge_mlp_v4(const float* P, int zero_row, const int* src, const u
                            const float* agg_logits, const float* agg_e_w, float* agg_h, int key_softmax, int sm_count, cudaStream_t st);
 void td_launch_rows_tc(int mode, const float* in, int ldi, int in_off, long long n_rows, TdMlp m, const unsigned char* w_image, int pieces, float* out,
                        int ldo, int nblocks, const int* row_list, const int* d_n_rows, int sm_count, cudaStream_t st);
+void td_launch_node_side_v4(const float* h, long long n_rows, const unsigned char* wn_img, const float* bn, const TdMlp& q_mlp, float* P,
+                            float* q, const int* rows, const int* d_n, int sm_count, cudaStream_t st);
 void td_launch_rel_compact(const unsigned char* flag, int n_nodes, int* rel_list, int* n_rel, cudaStream_t st);
 void td_launch_aggregate_h(const float* kbuf, const float* vbuf, const float* e_w, const int* src, const float* q, const float* h_in,
                            float* h_out, int n_nodes, int k, cudaStream_t st);
