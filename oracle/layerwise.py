@@ -109,8 +109,8 @@ def head(sd, lig_h, dtype=torch.float64):
 
 def block(sd, cfg, h, x, mask_ligand, batch_all, dtype=torch.float64):
     """One block of `restate.refine_net` from its input (h, x) [N,...] in the composed node order: the graph rebuilt from `x` as it
-    is (fp32 coordinates; `knn_graph_canonical` or `hybrid_graph`), the edge types, the global gate in `dtype`
-    (`global_edge_weight`), then the block's num_layers attention layers in `dtype`.  Returns (h, x, edge_index, e_w)."""
+    is (fp32 coordinates; `restate.connect_edge`: `knn_graph_canonical` or `hybrid_graph_canonical`), the edge types, the global
+    gate in `dtype` (`global_edge_weight`), then the block's num_layers attention layers in `dtype`.  Returns (h, x, edge_index, e_w)."""
     c = dict(DEFAULT_MODEL_CONFIG, **(cfg or {}))
     edge_index = restate.connect_edge(x.float(), c, mask_ligand, batch_all)
     edge_type = restate.build_edge_type(edge_index, mask_ligand).argmax(-1)

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from .synth import DEFAULT_MODEL_CONFIG, GAUSSIAN_OFFSETS
+from .synth import DEFAULT_MODEL_CONFIG, GAUSSIAN_OFFSETS, d2_fp32
 
 
 # ----------------------------------------------------------------------------------------------
@@ -159,7 +159,7 @@ def mlp(sd, prefix, x):
 # ----------------------------------------------------------------------------------------------
 def knn_graph_canonical(x, k, batch):
     """Canonical k-NN (SURVEY.md Appendix A.3): numpy, per graph, key = (fp32 d2, index) lexicographic.
-    d2 = ((dx*dx)+(dy*dy))+(dz*dz) with every op rounded to fp32.  Returns int64 [2,E] (row0 src, row1 dst)."""
+    d2 = ((dx*dx)+(dy*dy))+(dz*dz) with every op rounded to fp32 (`synth.d2_fp32`).  Returns int64 [2,E] (row0 src, row1 dst)."""
     xn = x.detach().cpu().numpy().astype(np.float32)
     bn = batch.detach().cpu().numpy()
     n = xn.shape[0]
@@ -169,11 +169,7 @@ def knn_graph_canonical(x, k, batch):
     for s, e in zip(starts, ends):
         xg = xn[s:e]
         ng = e - s
-        dx = xg[:, None, 0] - xg[None, :, 0]
-        dy = xg[:, None, 1] - xg[None, :, 1]
-        dz = xg[:, None, 2] - xg[None, :, 2]
-        d2 = ((dx * dx).astype(np.float32) + (dy * dy).astype(np.float32)).astype(np.float32)
-        d2 = (d2 + (dz * dz).astype(np.float32)).astype(np.float32)
+        d2 = d2_fp32(xg, xg)
         kk = min(k + 1, ng)
         idx = np.arange(ng)
         for i in range(ng):
@@ -186,11 +182,26 @@ def knn_graph_canonical(x, k, batch):
     return torch.from_numpy(np.stack([src, dst]).astype(np.int64))
 
 
-def hybrid_graph(x, k, mask_ligand, batch):
-    """cutoff_mode='hybrid' (models/uni_transformer.py:281-283 -> models/common.py:165-212, add_p_index=True).  Per graph, in this
-    edge order: ligand-ligand fully connected (dst-major, :167-171), for every ligand atom its k nearest PROTEIN atoms by
-    torch.norm distance / torch.topk (:174-182), and for protein destinations the ordinary k-NN over all atoms of the graph
-    (:196-203; nodes of a graph are protein atoms then ligand atoms after compose_context, so `all_index` is the identity)."""
+def _d2_fp32(a, b):
+    """synth.d2_fp32 on tensors."""
+    return d2_fp32(a.detach().cpu().numpy(), b.detach().cpu().numpy())
+
+
+def _nearest_protein_topk(x_lig, x_pro, k):
+    d = torch.norm(x_lig.unsqueeze(1) - x_pro.unsqueeze(0), p=2, dim=-1)               # common.py:174-175
+    return torch.topk(d, k=k, largest=False, dim=1).indices                            # :176
+
+
+def _nearest_protein_canonical(x_lig, x_pro, k):
+    if len(x_lig) and len(x_pro) < k:
+        raise RuntimeError('%d protein atoms < k = %d (torch.topk raises in the reference)' % (len(x_pro), k))
+    d2 = _d2_fp32(x_lig, x_pro)
+    idx = np.arange(len(x_pro))
+    order = [np.lexsort((idx, row))[:k] for row in d2]                                  # primary d2, secondary index
+    return torch.from_numpy(np.stack(order).astype(np.int64)) if len(x_lig) else torch.zeros(0, k, dtype=torch.long)
+
+
+def _hybrid(x, k, mask_ligand, batch, nearest_protein):
     B = int(batch.max().item()) + 1 if len(batch) else 0
     out = []
     for g in range(B):
@@ -200,8 +211,7 @@ def hybrid_graph(x, k, mask_ligand, batch):
         src = lig.repeat(len(lig))                                                      # :168
         keep = dst != src
         ll = torch.stack([src[keep], dst[keep]])
-        d = torch.norm(x[lig].unsqueeze(1) - x[pro].unsqueeze(0), p=2, dim=-1)         # :174-175
-        nn_p = pro[torch.topk(d, k=k, largest=False, dim=1).indices]                    # :176-177
+        nn_p = pro[nearest_protein(x[lig], x[pro], k)]                                  # :174-177
         pl = torch.stack([nn_p, lig.unsqueeze(1).repeat(1, k)], 0).view(2, -1)         # :178-182
         nodes = torch.cat([pro, lig])
         pe = knn_graph_canonical(x[nodes], k, torch.zeros(len(nodes), dtype=torch.long))   # :197
@@ -211,10 +221,27 @@ def hybrid_graph(x, k, mask_ligand, batch):
     return torch.cat(out, -1) if out else torch.zeros(2, 0, dtype=torch.long)
 
 
+def hybrid_graph(x, k, mask_ligand, batch):
+    """cutoff_mode='hybrid' (models/uni_transformer.py:281-283 -> models/common.py:165-212, add_p_index=True).  Per graph, in this
+    edge order: ligand-ligand fully connected (dst-major, :167-171), for every ligand atom its k nearest PROTEIN atoms by
+    torch.norm distance / torch.topk (:174-182), and for protein destinations the ordinary k-NN over all atoms of the graph
+    (:196-203; nodes of a graph are protein atoms then ligand atoms after compose_context, so `all_index` is the identity)."""
+    return _hybrid(x, k, mask_ligand, batch, _nearest_protein_topk)
+
+
+def hybrid_graph_canonical(x, k, mask_ligand, batch):
+    """`hybrid_graph` with the ligand rows' k nearest protein atoms chosen by the canonical k-NN key (fp32 d2, index) instead of
+    torch.norm / torch.topk.  The reference's topk breaks ties between equal torch.norm values in no specified order, and torch.norm
+    maps distinct fp32 d2 values to one float; the engine keeps the k smallest (d2, index) keys (DESIGN.md section 2).  Where no two
+    of the candidates around the k-th have equal torch.norm the two functions return the same edges in the same order."""
+    return _hybrid(x, k, mask_ligand, batch, _nearest_protein_canonical)
+
+
 def connect_edge(x, cfg, mask_ligand, batch):
-    """_connect_edge (models/uni_transformer.py:276-286); 'radius' is a dead path in the reference (undefined self.r)."""
+    """_connect_edge (models/uni_transformer.py:276-286); 'radius' is a dead path in the reference (undefined self.r).  The hybrid
+    graph is `hybrid_graph_canonical`: the reference's own `hybrid_graph` on every input where torch.topk's tie order is not reached."""
     if cfg['cutoff_mode'] == 'hybrid':
-        return hybrid_graph(x, cfg['knn'], mask_ligand, batch)
+        return hybrid_graph_canonical(x, cfg['knn'], mask_ligand, batch)
     return knn_graph_canonical(x, cfg['knn'], batch)
 
 

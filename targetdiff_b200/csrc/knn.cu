@@ -9,8 +9,10 @@
 //
 // cutoff_mode = 'hybrid' (reference models/common.py:165-212, add_p_index=True): protein destinations keep the k-NN over all atoms of
 // the graph; a ligand destination gets every other ligand atom of its graph (ascending node index) followed by its k nearest PROTEIN
-// atoms (same key order; the reference ranks torch.norm distances with torch.topk).  Rows have `stride` >= k slots (the engine uses
-// stride = k + max ligand atoms per graph - 1); unused slots are -1.
+// atoms by the same (d2, index) key.  The reference ranks torch.norm distances with torch.topk, whose order among equal norms is
+// unspecified, and distinct fp32 d2 can round to one norm: where such a tie falls at the k-th place the reference's choice differs
+// (DESIGN.md section 2, restate.hybrid_graph_canonical).  Rows have `stride` >= k slots (the engine uses stride = k + max ligand atoms
+// per graph - 1); unused slots are -1.
 //
 // Mapping: one CTA per (graph, chunk of queries); the graph's coordinates are staged once in shared memory
 // (coalesced float4 loads); one warp per query holds the key row in shared memory, each lane tracks the minimum of
