@@ -21,15 +21,16 @@
 //   * the epilogues work on the D fragment; only the key softmax and the fused aggregation exchange per-warp partials through a
 //     small shared-memory slot between the two warps that hold one destination's 32 rows.
 //
-// CTA = one producer warpgroup + kCons consumer warpgroups, one CTA per SM, persistent over tiles of 64 edge rows (one wgmma M).
-// The producer (one warp per consumer; `setmaxnreg` leaves it 40 registers and gives the consumers 232) stages each tile in shared
-// memory ahead of its consumer: the rows' metadata and the P[src] / P[dst] rows as 512-byte bulk copies.  Consumer c takes the CTA's tiles
-// c, c + kCons, ... and owns P stage c, which it hands back right after reading it (before its pre-MMA).  The two consumers'
-// tensor-core phases (pre-MMA, main MMA) run in a fixed alternating order (two named barriers): one consumer's MMAs are issued
-// whole while the other does its LayerNorm, split and epilogue, so the two never interleave on the tensor cores.
-// Shared memory: W2 pieces 64 KB | both class tables 64 KB | ln_b + b2 1 KB | exchange slots 4 KB per consumer |
-// 2 P stages of 39 KB (64 P[src] rows with a 544-byte stride, which makes the fragment-order reads free of bank conflicts,
-// kDst P[dst] rows, 64 metadata records) | mbarriers.  215 KB.
+// CTA = one producer warpgroup + kCons consumer warpgroups (3 for the unfolded NOUT = 128 launches, else 2: Map), one CTA per SM,
+// persistent over tiles of 64 edge rows (one wgmma M).  The producer (one warp per consumer; `setmaxnreg` leaves it 32 registers and
+// gives the consumers 160 with 3 consumers, 40 / 232 with 2) stages each tile in shared memory ahead of its consumer: the rows' metadata
+// and the P[src] / P[dst] rows as 512-byte bulk copies.  Consumer c takes the CTA's tiles c, c + kCons, ... and owns P stage c, which it
+// hands back right after reading it (before its pre-MMA).  With 2 consumers the tensor-core phases (pre-MMA, main MMA) run in a fixed
+// alternating order (named barriers): one consumer's MMAs are issued whole while the other does its LayerNorm, split and epilogue.
+// 3 consumers issue unordered (measured faster).  A launch covers one destination class, with that class's table resident.
+// Shared memory: W2 pieces 64 KB | the class table 32 KB | ln_b + b2 1 KB | exchange slots 4 KB per consumer |
+// kCons P stages of 39 KB (64 P[src] rows with a 544-byte stride, which makes the fragment-order reads free of bank conflicts,
+// kDst P[dst] rows, 64 metadata records) | mbarriers.  226 KB with 3 consumers.
 //
 // Folded key launch (FOLD, k = 32 or 64: a tile holds at most 2 destinations).  The key epilogue only needs
 //   logit[e, hd] = 1/sqrt(8) sum_d q[dst, 8 hd + d] (hid_e . W2^T + b2)[8 hd + d] = hid_e . M_dst[hd, :] + c_dst[hd],
@@ -50,11 +51,8 @@
 
 namespace v4 {
 
-constexpr int kCons = 2;                   // consumer warpgroups
-constexpr int kThreads = (kCons + 1) * 128;  // warpgroup 0 is the producer
 constexpr int kTile = 64;                  // rows per tile
 constexpr int kTabClassBytes = 2 * 128 * 128;   // one class table: 2 bf16 pieces of [128 x 64]
-constexpr int kProdRegs = 40, kConsRegs = 232;  // setmaxnreg: 128 * 40 + 2 * 128 * 232 = 384 * 168 (the launch's allocation)
 // P stage: P[src] rows (stride padded by 32 B: the 8 rows one fragment load touches fall in distinct banks), the tile's first kDst
 // destinations' P[dst] rows (k >= 8 never needs more; rows of further destinations, k <= 7, are read from global memory), and per row
 // the metadata record {node, src, dist, type | (dst slot + 1) << 8 | neighbour slot << 16}
@@ -62,17 +60,28 @@ constexpr int kSrcStride = 512 + 32, kDst = 8;
 constexpr int sSrc = 0, sDstRows = sSrc + kTile * kSrcStride, sMeta = sDstRows + kDst * 512, kStage = sMeta + kTile * 16;
 // folded key launch: per consumer the B image of M, 2 bf16 pieces of [32 rows x 128 K] (K halves of 32 x 128 B), and the 2 x 16 c_dst
 constexpr int kMAtom = 32 * 128, kMPiece = 2 * kMAtom, kMImg = 2 * kMPiece;
-// shared-memory map (bytes from the 1024-aligned base).  FOLD: W2 in fp32 instead of its bf16 image (both 64 KB), only the launch's
-// class table, plus the M images and c_dst.
-template <bool FOLD>
+// Per instantiation: the consumer count, the register split and the shared-memory map (bytes from the 1024-aligned base).  The
+// unfolded NOUT = 128 launches run three consumers; the folded key launch (its M images would need 274 KB with a third) and the h2x
+// xv launch keep two.  FOLD: W2 in fp32 instead of its bf16 image (both 64 KB), plus the M images and c_dst.
+template <int NOUT, bool FOLD>
 struct Map {
-  static constexpr int W = 0, T = W + 4 * 128 * 128, Par = T + (FOLD ? 1 : 2) * kTabClassBytes, X = Par + 2 * 128 * 4,
+  static constexpr int kCons = (NOUT == 128 && !FOLD) ? 3 : 2;   // consumer warpgroups
+  static constexpr int kThreads = (kCons + 1) * 128;              // warpgroup 0 is the producer
+  // setmaxnreg split of the launch's allocation: 3 consumers 128 * 32 + 3 * 128 * 160 = 512 * 128,
+  // 2 consumers 128 * 40 + 2 * 128 * 232 = 384 * 168
+  static constexpr int kProdRegs = kCons == 3 ? 32 : 40, kConsRegs = kCons == 3 ? 160 : 232;
+  static constexpr int W = 0, T = W + 4 * 128 * 128, Par = T + kTabClassBytes, X = Par + 2 * 128 * 4,
                        M = X + kCons * 4 * 2 * 128 * 4, C = M + (FOLD ? kCons * kMImg : 0), Stage = C + (FOLD ? kCons * 32 * 4 : 0),
                        Bar = Stage + kCons * kStage, Smem = Bar + 8 * (1 + 2 * kCons);   // barriers: weights, full[kCons], empty[kCons]
+  // MMA phase order (kernel comment): two consumers take turns; three issue unordered (measured faster than a ring on cfg3)
+  static constexpr bool kOrdered = kCons == 2;
+  // named barriers (0 is __syncthreads): 2 warp pairs per consumer, then per consumer its MMA-order barrier, then (FOLD) its
+  // M-image barrier
+  static constexpr int kPairBar = 1, kOrderBar = kPairBar + 2 * kCons, kFoldBar = kOrderBar + kCons;
   static_assert(M % 1024 == 0 && Stage % 128 == 0 && kStage % 128 == 0 && Smem <= 227 * 1024, "shared-memory map");
+  static_assert(128 * kProdRegs + kCons * 128 * kConsRegs == kThreads * (65536 / kThreads / 8 * 8), "register split");
+  static_assert(kFoldBar + kCons <= 16, "named barriers");
 };
-constexpr int kOrderBar = 5;               // named barriers kOrderBar + c: consumer c may issue its next MMA phase (1-4: warp pairs)
-constexpr int kFoldBar = 7;                // named barriers kFoldBar + c: consumer c's M image is written
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -154,21 +163,22 @@ using namespace v4;
 
 // NOUT = 128: key / value MLPs (hk, hv, xk);  NOUT = 16: the per-head scalar value MLP of h2x (xv).
 // Rows: idx = a * k + j over the destination list `row_nodes` (a < n_dst; entries < 0 are padding), edge slot e = row_nodes[a] * k + j.
-// Tiles below `split` destinations are protein-destination tiles (class table 0), the others ligand-destination tiles (table 1).
+// Destinations below `split` are protein destinations (class table 0), the others ligand destinations (table 1); a launch covers the
+// tiles of destination class `cls` only, with that class's table resident.
 //
 // Fragment ownership (thread t of warpgroup c, w = (t / 32) % 4, l = t % 32, q = l % 4): rows 16 w + l / 4 + 8 h (h = 0, 1), columns
 // 8 i + 2 q + {0, 1} (i < NOUT / 8) -- accumulator element d[4 i + 2 h + c] (hopper_mma.cuh).
-// FOLD (key MLPs, k = 32 or 64): the folded key path of the header; `w2_image` is then W2^T in fp32 ([128 f][128 out]) and the launch
-// covers the tiles of destination class `fold_cls` only (0: rows below split, 1: the rest).
+// FOLD (key MLPs, k = 32 or 64): the folded key path of the header; `w2_image` is then W2^T in fp32 ([128 f][128 out]).
 template <int NOUT, bool FOLD>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(Map<NOUT, FOLD>::kThreads, 1)
 edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restrict__ src, const unsigned char* __restrict__ etype,
                    const float* __restrict__ dist_arr, const int* __restrict__ row_nodes, long long n_dst, long long split_dst,
                    const int* __restrict__ d_counts, int k, int offA, int offB, const unsigned char* __restrict__ w2_image,
                    const unsigned char* __restrict__ tab_image, float coeff, const float* __restrict__ qnode, float* __restrict__ out, int out_by_slot, AggArgs agg,
-                   int fold_cls, const __grid_constant__ LnParams lp) {
+                   int cls, const __grid_constant__ LnParams lp) {
   static_assert(!FOLD || NOUT == 128, "the fold applies to the key MLPs");
-  using L = Map<FOLD>;
+  using L = Map<NOUT, FOLD>;
+  constexpr int kCons = L::kCons, kThreads = L::kThreads;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t sbase = smem_u32(smem_raw);
   const uint32_t sW = sbase + L::W, sT = sbase + L::T, sBar = sbase + L::Bar;
@@ -188,37 +198,31 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   if ((sbase & 1023u) != 0) __trap();            // SWIZZLE_128B atoms need a 1024-byte aligned window
   if (d_counts) { n_dst = d_counts[0]; split_dst = d_counts[1]; }      // destination subset compacted on the device
   const long long n_rows = n_dst * k, split_rows = split_dst * k;      // both multiples of 128 by construction of the lists
-  long long row_lo = 0, row_hi = n_rows;                               // the launch's rows: one class for FOLD, else all
-  if constexpr (FOLD) { if (fold_cls) row_lo = split_rows; else row_hi = split_rows; }
+  const long long row_lo = cls ? split_rows : 0, row_hi = cls ? n_rows : split_rows;   // the launch's rows: one destination class
   const long long n_tiles = row_hi > row_lo ? (row_hi - row_lo + kTile - 1) / kTile : 0;
   const long long my_tiles = (n_tiles > blockIdx.x) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
   // P stage c: full[c] (producer -> consumer c, 32 producer lanes + the bytes of the copies), empty[c] (consumer c's 128 threads)
   auto full_bar = [&](int c) { return sBar + 8u * (1 + c); };
   auto empty_bar = [&](int c) { return sBar + 8u * (1 + kCons + c); };
 
-  // ---- one-time setup: weight image and both class tables -> smem (TMA bulk copies), bias vectors -> smem
+  // ---- one-time setup: weight image and the launch's class table -> smem (TMA bulk copies), bias vectors -> smem
   constexpr int kWAtom = NOUT * 128;            // one K-half of a weight piece: NOUT rows x 128 B
   constexpr int kWPiece = 2 * kWAtom;
+  constexpr uint32_t kWBytes = FOLD ? 4u * 128 * 128 : 2u * kWPiece;   // FOLD: W2^T fp32 (the same 64 KB as the two bf16 pieces)
   if (tid == 0) {
     mbar_init(sBar, 1);
     for (int c = 0; c < kCons; ++c) { mbar_init(full_bar(c), 32); mbar_init(empty_bar(c), 128); }
     fence_barrier_init();
-    if constexpr (FOLD) {                       // W2^T fp32 (the same 64 KB as the two bf16 pieces) and this launch's class table
-      mbar_expect_tx(sBar, 4u * 128 * 128 + kTabClassBytes);
-      bulk_g2s(sW, w2_image, 4u * 128 * 128, sBar);
-      bulk_g2s(sT, tab_image + (size_t)fold_cls * kTabClassBytes, kTabClassBytes, sBar);
-    } else {
-      mbar_expect_tx(sBar, 2u * kWPiece + 2u * kTabClassBytes);
-      bulk_g2s(sW, w2_image, 2u * kWPiece, sBar);
-      bulk_g2s(sT, tab_image, 2u * kTabClassBytes, sBar);
-    }
+    mbar_expect_tx(sBar, kWBytes + kTabClassBytes);
+    bulk_g2s(sW, w2_image, kWBytes, sBar);
+    bulk_g2s(sT, tab_image + (size_t)cls * kTabClassBytes, kTabClassBytes, sBar);
   }
   for (int i = tid; i < 128; i += kThreads) { s_b[i] = lp.b[i]; s_b2[i] = lp.b2[i]; }
   __syncthreads();
 
   if (warp < 4) {
     // ================================================================= producer
-    setmaxnreg_dec<kProdRegs>();
+    setmaxnreg_dec<L::kProdRegs>();
     // producer warp c fills stage c for consumer c.  A tile's metadata is gathered before the wait for the stage, so only the bulk
     // copies remain between the consumer's hand-back and its next tile.
     if (warp >= kCons) return;
@@ -269,7 +273,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   }
 
   // ================================================================= consumers
-  setmaxnreg_inc<kConsRegs>();
+  setmaxnreg_inc<L::kConsRegs>();
   const int cwg = (warp >> 2) - 1;
   float mu[5];
 #pragma unroll
@@ -278,7 +282,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   mbar_wait(sBar, 0);
 
   const int r_base = 16 * w + (lane >> 2);
-  const int pair_bar = 1 + 2 * cwg + (w >> 1);                  // named barrier of the warp pair {w & 2, (w & 2) + 1}
+  const int pair_bar = L::kPairBar + 2 * cwg + (w >> 1);        // named barrier of the warp pair {w & 2, (w & 2) + 1}
   float* const xslot = reinterpret_cast<float*>(smem_raw + L::X) + (size_t)(cwg * 4 + w) * 256;   // 2 sets x 128; partner at (w ^ 1)
   float* const xpart = xslot + ((w & 1) ? -256 : 256);
   const bool do_agg = !FOLD && NOUT == 128 && qnode == nullptr && agg.logits != nullptr;
@@ -292,23 +296,26 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
   unsigned char* const mimg = smem_raw + L::M + cwg * kMImg;
   float* const s_c = reinterpret_cast<float*>(smem_raw + L::C) + cwg * 32;      // c_dst[slot][head]
   const int srow = k == 32 ? (w >> 1) : 0;                                        // FOLD: destination slot of this warp's rows
-  // MMA phase order: consumer 0 first, then strictly alternating.  Every consumer runs the same number of iterations (one without
-  // a tile only passes the order on); consumer 1's first hand-over and consumer 0's wait after the loop keep the counts equal, so
-  // no barrier is left half-arrived.
-  const int order_mine = kOrderBar + cwg, order_other = kOrderBar + (cwg ^ 1);
+  // MMA phase order (kOrdered), a ring: consumer 0 first, then 1, ..., kCons - 1, 0, ...  Consumer c waits on its own barrier and
+  // hands over on that of c + 1 (mod kCons).  Every consumer runs the same number of iterations (one without a tile only passes the
+  // order on); the last consumer's first hand-over and consumer 0's wait after the loop keep the counts equal, so no barrier is left
+  // half-arrived.
+  const int order_mine = L::kOrderBar + cwg, order_next = L::kOrderBar + (cwg + 1) % kCons;
+  auto order_wait = [&] { if constexpr (L::kOrdered) named_bar_sync(order_mine, 256); };
+  auto order_pass = [&] { if constexpr (L::kOrdered) named_bar_arrive(order_next, 256); };
   const long long n_iter = (my_tiles + kCons - 1) / kCons;
   if (n_iter == 0) return;
-  if (cwg == 1) named_bar_arrive(order_other, 256);
+  if (cwg == kCons - 1) order_pass();
   int set = 0;
 
   for (long long n = 0; n < n_iter; ++n, set ^= 1) {
     const long long it = n * kCons + cwg;
     if (it >= my_tiles) {
-      for (int phase = 0; phase < 2; ++phase) { named_bar_sync(order_mine, 256); named_bar_arrive(order_other, 256); }
+      if constexpr (L::kOrdered)
+        for (int phase = 0; phase < 2; ++phase) { order_wait(); order_pass(); }
       continue;
     }
-    const long long tile = blockIdx.x + it * (long long)gridDim.x, row0 = row_lo + tile * kTile;
-    const int cls = FOLD ? 0 : (row0 >= split_rows) ? 1 : 0;       // FOLD: the one resident table
+    const long long row0 = row_lo + (blockIdx.x + it * (long long)gridDim.x) * kTile;
     // ---- metadata of this thread's two rows (s < 0: absent edge / padding destination / beyond the end)
     long long idx[2];
     int node[2], s[2], ty[2], jj[2], dsl[2];
@@ -388,18 +395,17 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       }
     }
     mbar_arrive(empty_bar(cwg));                                  // P stage read: the producer may refill it
-    const uint32_t sTc = sT + (uint32_t)cls * kTabClassBytes;
     wgmma_fence();
-    named_bar_sync(order_mine, 256);
+    order_wait();
 #pragma unroll
     for (int term = 0; term < 3; ++term) {
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk)
-        wgmma_n128_rs(x, term == 2 ? glo[kk] : ghi[kk], gmma_desc_sw128(sTc + (term == 1 ? kTabClassBytes / 2 : 0) + kk * 32),
+        wgmma_n128_rs(x, term == 2 ? glo[kk] : ghi[kk], gmma_desc_sw128(sT + (term == 1 ? kTabClassBytes / 2 : 0) + kk * 32),
                       1u);                        // a1b1, a1b2, a2b1
     }
     wgmma_commit();
-    named_bar_arrive(order_other, 256);
+    order_pass();
     if constexpr (FOLD) {
       // ---- while the pre-MMA runs: M rows fn0 (slot 0) and fn0 + 8 (slot 1) over this thread's two K runs, split into two bf16
       //      pieces and stored in the K-major SWIZZLE_128B image (the previous tile's main MMA has completed in every warp: they all
@@ -478,7 +484,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
     // ---- D = hid . W2^T   (FOLD: D = c_dst + hid . M^T, N = 32; o[4 i + 2 h + c] is head 4 q + 2 (i / 2) + c of slot i % 2)
     float o[NOUT / 2];
     if constexpr (FOLD) {
-      named_bar_sync(kFoldBar + cwg, 128);                          // M image and c_dst written by all 4 warps
+      named_bar_sync(L::kFoldBar + cwg, 128);                        // M image and c_dst written by all 4 warps
 #pragma unroll
       for (int sl = 0; sl < 2; ++sl) {
         const float4 cv = *reinterpret_cast<const float4*>(s_c + 16 * sl + 4 * q);
@@ -490,7 +496,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       }
     }
     wgmma_fence();
-    named_bar_sync(order_mine, 256);
+    order_wait();
 #pragma unroll
     for (int term = 0; term < 3; ++term) {
 #pragma unroll
@@ -506,7 +512,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       }
     }
     wgmma_commit();
-    named_bar_arrive(order_other, 256);
+    order_pass();
     wgmma_wait_all();
 
     // ================================================================= epilogue on the D fragment
@@ -529,9 +535,9 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
             stg64(out + (size_t)orow[h] * 16 + 8 * i + 2 * q, o[4 * i + 2 * h] + bb.x, o[4 * i + 2 * h + 1] + bb.y);
           }
     } else if (do_agg) {
-      // ---- value MLP with the attention aggregation fused in: the warp pair's 32 rows are the edges of destination `dnode`
-      const long long dslot = tile * 2 + (w >> 1);
-      const int dnode = dslot < n_dst ? row_nodes[dslot] : -1;        // warp-uniform
+      // ---- value MLP with the attention aggregation fused in: the warp pair's 32 rows are the edges of destination `dnode`, the
+      //      staged node of each of them (-1: padding destination or beyond the end)
+      const int dnode = node[0];                                      // warp-uniform
       const bool active = dnode >= 0;
       const int ccol = 64 * (w & 1) + 2 * lane;                       // the two h columns this lane writes
       float2 hin = make_float2(0.f, 0.f);
@@ -664,7 +670,7 @@ edge_mlp_v4_kernel(const float* __restrict__ P, int zero_row, const int* __restr
       }
     }
   }
-  if (cwg == 0) named_bar_sync(order_mine, 256);                 // matches consumer 1's last hand-over
+  if (cwg == 0) order_wait();                                    // matches the last consumer's last hand-over
 }
 
 // n_dst destinations (device counts {n_dst, split_dst} in d_counts override the host values); see the kernel comment for the row model
@@ -679,31 +685,31 @@ void td_launch_edge_mlp_v4(const float* P, int zero_row, const int* src, const u
   memcpy(lp.b2, h_b2, sizeof(float) * (size_t)m.nout);
   memcpy(lp.mu, h_offsets, sizeof(lp.mu));
   static size_t opted128[TD_MAX_DEVICES] = {0}, opted16[TD_MAX_DEVICES] = {0}, optedF[TD_MAX_DEVICES] = {0};
-  td_opt_in_smem(edge_mlp_v4_kernel<128, false>, Map<false>::Smem, opted128);
-  td_opt_in_smem(edge_mlp_v4_kernel<16, false>, Map<false>::Smem, opted16);
-  td_opt_in_smem(edge_mlp_v4_kernel<128, true>, Map<true>::Smem, optedF);
-  auto grid_of = [&](long long n_dst_range) {                         // with d_counts: upper bound
-    const long long n_tiles = (n_dst_range * k + kTile - 1) / kTile;
-    return (int)(n_tiles < sm_count ? n_tiles : sm_count);
-  };
+  td_opt_in_smem(edge_mlp_v4_kernel<128, false>, Map<128, false>::Smem, opted128);
+  td_opt_in_smem(edge_mlp_v4_kernel<16, false>, Map<16, false>::Smem, opted16);
+  td_opt_in_smem(edge_mlp_v4_kernel<128, true>, Map<128, true>::Smem, optedF);
   AggArgs agg = {agg_logits, agg_e_w, agg_h, (key_softmax && k == 32) ? 1 : 0};
-  if (m.nout == 16) {
-    edge_mlp_v4_kernel<16, false><<<grid_of(n_dst), kThreads, Map<false>::Smem, st>>>(
-        P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB, m.w2_img, m.tabcls_img, coeff, nullptr, out,
-        out_by_slot, agg, 0, lp);
-  } else if (qnode && (k == 32 || k == 64)) {
-    // folded key launch, one per destination class (a tile then holds at most 2 destinations); the host split bounds the device one
-    // from above and the ligand part is the same on both, so a class the host counts as empty is empty on the device too
-    const long long n_cls[2] = {split_dst, n_dst - split_dst};
-    for (int cls = 0; cls < 2; ++cls)
-      if (n_cls[cls] > 0)
-        edge_mlp_v4_kernel<128, true><<<grid_of(n_cls[cls]), kThreads, Map<true>::Smem, st>>>(
-            P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB,
-            reinterpret_cast<const unsigned char*>(m.w2t), m.tabcls_img, coeff, qnode, out, out_by_slot, agg, cls, lp);
-  } else {
-    // k <= 31 or k = 48: a tile spans more destinations than the N = 32 fold has slots for; keys are computed whole
-    edge_mlp_v4_kernel<128, false><<<grid_of(n_dst), kThreads, Map<false>::Smem, st>>>(
-        P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB, m.w2_img, m.tabcls_img, coeff, qnode, out,
-        out_by_slot, agg, 0, lp);
+  // the folded key launch needs a tile to hold at most 2 destinations (k = 32 or 64); for k <= 31 or k = 48 keys are computed whole
+  const bool fold = m.nout == 128 && qnode && (k == 32 || k == 64);
+  // One launch per destination class (protein destinations, then ligand destinations), so that one class table is resident.  With
+  // device counts the host split bounds the device one from above and the ligand part is the same on both: a class the host counts
+  // as empty is empty on the device too, and the host counts give each launch an upper bound on its tiles.
+  const long long n_cls[2] = {split_dst, n_dst - split_dst};
+  for (int cls = 0; cls < 2; ++cls) {
+    if (n_cls[cls] == 0) continue;
+    const long long n_tiles = (n_cls[cls] * k + kTile - 1) / kTile;
+    const int grid = (int)(n_tiles < sm_count ? n_tiles : sm_count);
+    if (m.nout == 16)
+      edge_mlp_v4_kernel<16, false><<<grid, Map<16, false>::kThreads, Map<16, false>::Smem, st>>>(
+          P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB, m.w2_img, m.tabcls_img, coeff, nullptr,
+          out, out_by_slot, agg, cls, lp);
+    else if (fold)
+      edge_mlp_v4_kernel<128, true><<<grid, Map<128, true>::kThreads, Map<128, true>::Smem, st>>>(
+          P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB,
+          reinterpret_cast<const unsigned char*>(m.w2t), m.tabcls_img, coeff, qnode, out, out_by_slot, agg, cls, lp);
+    else
+      edge_mlp_v4_kernel<128, false><<<grid, Map<128, false>::kThreads, Map<128, false>::Smem, st>>>(
+          P, zero_row, src, etype, dist, row_nodes, n_dst, split_dst, d_counts, k, m.offA, m.offB, m.w2_img, m.tabcls_img, coeff, qnode,
+          out, out_by_slot, agg, cls, lp);
   }
 }
