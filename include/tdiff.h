@@ -146,6 +146,25 @@ TDIFF_API int tdiff_get_node_pos(tdiff_engine* e, float* d_x, void* stream);
 TDIFF_API int tdiff_sample(tdiff_engine* e, int num_steps, const float* d_pos_noise, const float* d_v_uniform, uint64_t seed,
                  float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only, void* stream);
 
+/* Fixed atoms (fragment-conditioned sampling; an extension beyond the reference, DESIGN.md section 1).  Ligand atoms with
+ * d_mask[a] != 0 are held to the forward process of a target (x0_f, v0_f) through every later tdiff_sample: before the first step
+ * they are set to a sample of q(x_{T-1} | x0_f), q(v_{T-1} | v0_f); after the step at time t (whose network sees every atom and
+ * whose posterior update runs for every row) they are overwritten with a fresh sample of q(x_{t-1} | x0_f), q(v_{t-1} | v0_f), or
+ * with x0_f, v0_f exactly after t = 0.  Position sqrt(alphas_cumprod) x0_f + sqrt(1 - alphas_cumprod) eps; type Gumbel-max over
+ * q_v_pred(log_onehot(v0_f)).  d_pos_traj / d_v_traj record the state after the overwrite, d_v0_traj / d_vt_traj what the network and
+ * the posterior produced.  With pos_only the types of every row are left as they are.  tdiff_forward and the other calls ignore it.
+ * d_mask [Nl] uint8, or NULL to clear the set; d_pos0 [Nl,3] fp32 (lab frame if apply_center != 0, centred otherwise) and d_v0 [Nl]
+ * int64 are read at masked rows only (class >= num_classes -> TDIFF_EINVAL; synchronises the stream).  Before tdiff_bind_batch ->
+ * TDIFF_ESTATE; tdiff_bind_batch clears the set.  Costs one extra launch per chain and none per step.
+ * Noise: without tapes, draw d (d = 0 before the first step, d = j + 1 after step j) comes from the same Philox key as the sampler
+ * on its own counters (a, d, 0, 0x66787073) for positions and (a, d, 1 + c/4, 0x66787476) for class c; the free atoms' stream is
+ * unchanged.  tdiff_set_fixed_tape gives those draws as a tape instead: d_pos_noise [S+1,Nl,3], d_v_uniform [S+1,Nl,K] (NULL under
+ * pos_only) for the next chains of num_steps = S (borrowed pointers, NULL clears, tdiff_bind_batch clears).  With a fixed set, a chain
+ * takes either both tapes or neither (TDIFF_EINVAL otherwise), so the two sources of noise are never mixed. */
+TDIFF_API int tdiff_set_fixed(tdiff_engine* e, const uint8_t* d_mask, const float* d_pos0, const int64_t* d_v0, int apply_center,
+                              void* stream);
+TDIFF_API int tdiff_set_fixed_tape(tdiff_engine* e, const float* d_pos_noise, const float* d_v_uniform);
+
 /* Same loop through HOST buffers (the end-to-end path: H2D of the inputs, the chain, D2H of the results, all on
  * `stream`, synchronised before returning).  Equivalent of the device-facing part of sample_diffusion_ligand
  * (scripts/sample_diffusion.py:42-112) for one batch.  h_out_* may be NULL. */

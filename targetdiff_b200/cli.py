@@ -1,7 +1,11 @@
 """Command line for the sampling path (same arguments / outputs as the reference's scripts).
 
     python -m targetdiff_b200.cli sample_for_pocket configs/sampling.yml --pdb_path pocket.pdb [--num_samples N] [--result_path DIR]
-        (reference scripts/sample_for_pocket.py:34-93: sample ligands into one pocket given as a PDB file)
+            [--fragment FILE]
+        (reference scripts/sample_for_pocket.py:34-93: sample ligands into one pocket given as a PDB file; --fragment FILE, a .pt or
+        .npz holding 'pos' [n,3] (the PDB's frame) and 'v' [n] class indices, grows every sample from that fragment: its atoms are
+        the first n of each ligand and end exactly at 'pos' / 'v', see targetdiff_b200.sampling.  sample.pt then also holds
+        'fixed_ligand_atoms': n)
 
     [torchrun --nproc-per-node N -m] python -m targetdiff_b200.cli sample_pockets configs/sampling.yml --pocket_dir DIR | --pocket_list FILE
             [-i ID] [--schedule round_robin|longest_first] [--result_path DIR] [--num_samples N] [--batch_size B]
@@ -129,6 +133,26 @@ def sample_pockets(argv):
     return done
 
 
+def load_fragment(path):
+    """(pos float32 [n,3], v int64 [n]) from a .pt (a dict) or .npz file with entries 'pos' and 'v'."""
+    if path.endswith('.npz'):
+        import numpy as np
+        with np.load(path) as z:
+            d = {k: z[k] for k in z.files}
+    elif path.endswith('.pt'):
+        d = torch.load(path, map_location='cpu', weights_only=True)
+    else:
+        raise ValueError('--fragment %s: expected a .pt or .npz file' % path)
+    if not isinstance(d, dict) or 'pos' not in d or 'v' not in d:
+        raise ValueError("--fragment %s must hold 'pos' [n,3] and 'v' [n]" % path)
+    pos = torch.as_tensor(d['pos']).float()
+    v = torch.as_tensor(d['v'])
+    if v.is_floating_point() or pos.dim() != 2 or pos.shape[1] != 3 or v.dim() != 1 or v.shape[0] != pos.shape[0] or v.shape[0] < 1:
+        raise ValueError("--fragment %s: 'pos' must be [n,3] and 'v' [n] integer class indices (n >= 1), got %s and %s %s"
+                         % (path, tuple(pos.shape), tuple(v.shape), v.dtype))
+    return pos, v.long()
+
+
 def sample_for_pocket(argv):
     ap = argparse.ArgumentParser(prog='targetdiff_b200.cli sample_for_pocket')
     ap.add_argument('config', type=str)
@@ -137,18 +161,23 @@ def sample_for_pocket(argv):
     ap.add_argument('--batch_size', type=int, default=100)
     ap.add_argument('--result_path', type=str, default='./outputs_pdb')
     ap.add_argument('--num_samples', type=int)
+    ap.add_argument('--fragment', type=str, help=".pt / .npz with 'pos' [n,3] and 'v' [n]: every sample grows from this fragment")
     a = ap.parse_args(argv)
     config = load_config(a.config)
+    fragment = load_fragment(a.fragment) if a.fragment else None
     seed_all(config.sample.seed)
     model = _load_model(config, a.device)
     data = pdb_to_pocket_data(a.pdb_path)
     n = a.num_samples if a.num_samples is not None else config.sample.num_samples
     outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=a.device, num_steps=config.sample.num_steps,
                                       pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
-                                      sample_num_atoms=config.sample.sample_num_atoms)
+                                      sample_num_atoms=config.sample.sample_num_atoms, fixed_ligand=fragment)
     os.makedirs(a.result_path, exist_ok=True)
     shutil.copyfile(a.config, os.path.join(a.result_path, 'sample.yml'))
-    torch.save(build_result(data, outputs), os.path.join(a.result_path, 'sample.pt'))
+    result = build_result(data, outputs)
+    if fragment is not None:
+        result['fixed_ligand_atoms'] = int(fragment[1].shape[0])
+    torch.save(result, os.path.join(a.result_path, 'sample.pt'))
     print('Sample done! %d molecules, %.1f s' % (len(outputs[0]), sum(outputs[-1])))
 
 

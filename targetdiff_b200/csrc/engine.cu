@@ -90,7 +90,7 @@ struct tdiff_engine {
   DevBuf h_sync;                            // sync_twoup: the layer's input h, read by its h2x sub-layers
   const float *hd_w1t = nullptr, *hd_b1 = nullptr, *hd_w2 = nullptr, *hd_b2 = nullptr;
   const float *t_c0 = nullptr, *t_ct = nullptr, *t_logvar = nullptr, *t_la = nullptr, *t_l1ma = nullptr, *t_lca = nullptr, *t_l1mca = nullptr,
-              *t_sra = nullptr, *t_srm1 = nullptr;
+              *t_sra = nullptr, *t_srm1 = nullptr, *t_ac = nullptr;
   // ---- batch
   bool bound = false, has_ligand = false, have_graph = false;
   bool restrict_last = false;           // sampling loop only: the last layer's x2h is evaluated for the relevant nodes only
@@ -120,6 +120,10 @@ struct tdiff_engine {
   long long free_stride = 0;            // ints per cached evaluation in free_rows
   DevBuf xm0, xm1, offset, h0, h, P, q, src, src_prev, etype, e_w, dist, kbuf, vbuf, v16, lig_pos, lig_v, logits;
   DevBuf step, err_flag, node_off, total_edges;
+  // fixed atoms (tdiff_set_fixed / tdiff_set_fixed_tape); cleared by tdiff_bind_batch
+  bool has_fixed = false;
+  DevBuf fix_mask, fix_pos, fix_v;
+  const float *fix_pos_noise = nullptr, *fix_v_uniform = nullptr;
   DevBuf stage[8];   // staging for tdiff_sample_host
   // ---- instrumentation
   cudaStream_t own_stream = nullptr;   // capture stream (the caller's stream may be the legacy default stream, which cannot capture)
@@ -439,9 +443,9 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
   for (int i = 0; i < n_entries; ++i)
     if (sd[i].name) pk.byname[sd[i].name] = &sd[i];
   const int T = cfg->num_timesteps, KC = cfg->num_classes, F = cfg->protein_feat_dim, L = cfg->num_layers;
-  struct { const char* name; size_t off; } tabs[9] = {{"posterior_mean_c0_coef", 0}, {"posterior_mean_ct_coef", 0}, {"posterior_logvar", 0},
+  struct { const char* name; size_t off; } tabs[10] = {{"posterior_mean_c0_coef", 0}, {"posterior_mean_ct_coef", 0}, {"posterior_logvar", 0},
       {"log_alphas_v", 0}, {"log_one_minus_alphas_v", 0}, {"log_alphas_cumprod_v", 0}, {"log_one_minus_alphas_cumprod_v", 0},
-      {"sqrt_recip_alphas_cumprod", 0}, {"sqrt_recipm1_alphas_cumprod", 0}};
+      {"sqrt_recip_alphas_cumprod", 0}, {"sqrt_recipm1_alphas_cumprod", 0}, {"alphas_cumprod", 0}};
   for (auto& t : tabs) {
     const float* p = pk.get(t.name, T);
     t.off = pk.alloc(T);
@@ -553,7 +557,7 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
   const unsigned char* IM = e->img_arena;
   e->t_c0 = A + tabs[0].off; e->t_ct = A + tabs[1].off; e->t_logvar = A + tabs[2].off; e->t_la = A + tabs[3].off;
   e->t_l1ma = A + tabs[4].off; e->t_lca = A + tabs[5].off; e->t_l1mca = A + tabs[6].off;
-  e->t_sra = A + tabs[7].off; e->t_srm1 = A + tabs[8].off;
+  e->t_sra = A + tabs[7].off; e->t_srm1 = A + tabs[8].off; e->t_ac = A + tabs[9].off;
   e->w_prot = A + o_wp; e->b_prot = A + o_bp; e->wl_t = A + o_wl; e->bl = A + o_bl;
   e->w_time = cfg->time_emb ? A + o_wtime : nullptr; e->zeros128 = A + o_zeros;
   e->ew_w1t = A + o_gw1; e->ew_b1 = A + o_gb1; e->ew_g = A + o_gg; e->ew_b = A + o_gb; e->ew_w2 = A + o_gw2; e->ew_off = A + o_goff;
@@ -600,7 +604,7 @@ extern "C" void tdiff_destroy(tdiff_engine* e) {
   if (e->ev_join) cudaEventDestroy(e->ev_join);
   DevBuf* bufs[] = {&e->node_ptr, &e->prot_ptr, &e->prot_node, &e->prot_graph, &e->lig_node, &e->lig_graph, &e->node_lig, &e->xm0, &e->xm1,
                     &e->rel_flag, &e->rel_list, &e->n_rel, &e->work_list, &e->n_work, &e->knn_cache, &e->x2h_rows, &e->lig_rows, &e->rel_rows, &e->rel_counts, &e->ew_x2h, &e->ew_h2x, &e->h_sync, &e->hagg, &e->time_norm, &e->h_free, &e->dirty, &e->free_rows, &e->free_counts, &e->lig_save, &e->offset, &e->h0, &e->h, &e->P, &e->q, &e->src, &e->src_prev, &e->etype, &e->e_w, &e->dist, &e->kbuf, &e->vbuf, &e->v16, &e->lig_pos,
-                    &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges};
+                    &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges, &e->fix_mask, &e->fix_pos, &e->fix_v};
   for (auto* b : bufs) b->release();
   for (auto& b : e->stage) b.release();
   if (e->arena) cudaFree(e->arena);
@@ -651,6 +655,7 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   }
   node_ptr[B] = n; prot_ptr[B] = p;
   e->bound = false; e->has_ligand = false; e->have_graph = false; e->have_prev = false;
+  e->has_fixed = false; e->fix_pos_noise = nullptr; e->fix_v_uniform = nullptr;
   e->B = B; e->N = (int)N; e->Np = (int)Np; e->Nl = (int)Nl; e->max_ng = max_ng;
   const size_t slots = (size_t)N * K;
   int bad = 0;
@@ -759,6 +764,41 @@ extern "C" int tdiff_set_ligand(tdiff_engine* e, const float* d_pos, const int64
   }
   CK(cudaGetLastError());
   e->has_ligand = true;
+  return TDIFF_OK;
+}
+
+extern "C" int tdiff_set_fixed(tdiff_engine* e, const uint8_t* d_mask, const float* d_pos0, const int64_t* d_v0, int apply_center, void* stream) {
+  if (!e || !e->bound) return set_err(TDIFF_ESTATE, "set_fixed before bind_batch");
+  if (!d_mask) {
+    e->has_fixed = false;
+    return TDIFF_OK;
+  }
+  if (e->Nl > 0 && (!d_pos0 || !d_v0)) return set_err(TDIFF_EINVAL, "set_fixed: a mask needs target positions and classes");
+  cudaStream_t st = (cudaStream_t)stream;
+  CK(cudaSetDevice(e->device));
+  const size_t Nl = (size_t)e->Nl;
+  if (e->fix_mask.ensure(Nl + 16) | e->fix_pos.ensure(Nl * 16 + 16) | e->fix_v.ensure(Nl * 4 + 16))
+    return set_err(TDIFF_ECUDA, "out of device memory for the fixed set of %zu ligand atoms", Nl);
+  e->has_fixed = false;
+  td_launch_set_fixed(d_mask, d_pos0, (const long long*)d_v0, e->lig_graph.as<int>(), e->offset.as<float4>(), apply_center, e->Nl,
+                      e->cfg.num_classes, e->fix_mask.as<unsigned char>(), e->fix_pos.as<float4>(), e->fix_v.as<int>(), e->err_flag.as<int>(), st);
+  e->launches += 1;
+  int flag = 0;
+  CK(cudaMemcpyAsync(&flag, e->err_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (flag) {
+    cudaMemsetAsync(e->err_flag.p, 0, sizeof(int), st);
+    return set_err(TDIFF_EINVAL, "fixed atom class index outside 0..%d", e->cfg.num_classes - 1);
+  }
+  CK(cudaGetLastError());
+  e->has_fixed = true;
+  return TDIFF_OK;
+}
+
+extern "C" int tdiff_set_fixed_tape(tdiff_engine* e, const float* d_pos_noise, const float* d_v_uniform) {
+  if (!e || !e->bound) return set_err(TDIFF_ESTATE, "set_fixed_tape before bind_batch");
+  e->fix_pos_noise = d_pos_noise;
+  e->fix_v_uniform = d_pos_noise ? d_v_uniform : nullptr;
   return TDIFF_OK;
 }
 
@@ -1145,6 +1185,13 @@ extern "C" int tdiff_sample(tdiff_engine* e, int num_steps, const float* d_pos_n
   if (num_steps < 0 || num_steps > T) return set_err(TDIFF_EINVAL, "num_steps=%d outside 0..%d", num_steps, T);
   if ((d_pos_noise == nullptr) != (d_v_uniform == nullptr) && !pos_only)
     return set_err(TDIFF_EINVAL, "noise tape needs both pos_noise and v_uniform (or neither for Philox)");
+  if (e->has_fixed) {      // one noise source per chain: both tapes or neither
+    if ((d_pos_noise != nullptr) != (e->fix_pos_noise != nullptr))
+      return set_err(TDIFF_EINVAL, d_pos_noise ? "fixed atoms with a noise tape need a fixed-atom tape (tdiff_set_fixed_tape)"
+                                               : "a fixed-atom tape is set but the chain has no noise tape (clear it, or pass both)");
+    if (d_pos_noise && !pos_only && !e->fix_v_uniform)
+      return set_err(TDIFF_EINVAL, "the fixed-atom tape needs v_uniform unless pos_only");
+  }
   cudaStream_t st = (cudaStream_t)stream;
   CK(cudaSetDevice(e->device));
   if (num_steps == 0) return TDIFF_OK;
@@ -1159,7 +1206,15 @@ extern "C" int tdiff_sample(tdiff_engine* e, int num_steps, const float* d_pos_n
   A.pos_noise = d_pos_noise; A.v_uniform = d_v_uniform; A.seed = seed;
   A.lig_pos = e->lig_pos.as<float4>(); A.lig_v = e->lig_v.as<int>();
   A.pos_traj = d_pos_traj; A.v_traj = (long long*)d_v_traj; A.v0_traj = d_v0_traj; A.vt_traj = d_vt_traj;
+  if (e->has_fixed) {
+    A.fix_mask = e->fix_mask.as<unsigned char>(); A.fix_pos = e->fix_pos.as<float4>(); A.fix_v = e->fix_v.as<int>(); A.ac = e->t_ac;
+    A.fix_pos_noise = e->fix_pos_noise; A.fix_v_uniform = e->fix_v_uniform;
+  }
   CK(cudaMemsetAsync(e->step.p, 0, sizeof(int), st));
+  if (e->has_fixed) {      // the chain's one extra launch: fixed rows <- q(x_{T-1} | x0_f), q(v_{T-1} | v0_f)
+    td_launch_fixed_init(A, st);
+    e->launches += 1;
+  }
   if (e->free_depth > 0 && !e->free_ready) build_free_cache(e, st);
   const bool eager = e->profiling || e->env_no_graph;
   Prof* total = new Prof(e, st, EV_TOTAL);

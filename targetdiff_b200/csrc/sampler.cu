@@ -28,12 +28,73 @@ __device__ __forceinline__ float log_add_exp_f(float a, float b) {
   return mx + logf(expf(a - mx) + expf(b - mx));
 }
 
+// Philox domain words of the fixed-atom stream ("fxps", "fxtv"), distinct from the sampler's "pst\0" / "vuni" (oracle/fixed_atoms.py)
+#define TD_FIX_POS_DOMAIN 0x66787073u
+#define TD_FIX_TYPE_DOMAIN 0x66787476u
+
+// Fixed atom `a` (DESIGN.md section 1, fixed atoms): a sample of q(x_tm | x0_f) and q(v_tm | v0_f) from draw `d` of the fixed-atom
+// stream (d = 0 before the first step, d = j + 1 after step j), or x0_f / v0_f exactly when tm < 0.  Position
+// sqrt(ac) x0 + sqrt(1 - ac) eps with every product and the sum rounded once, as the reference's perturbation
+// (models/molopt_score_model.py:500-504); type: Gumbel-max over the unnormalised q_v_pred(log_onehot(v0), tm) (q_v_sample, :394-398).
+// With pos_only the type is left as it is.
+__device__ __forceinline__ void fixed_sample(const TdStepArgs& A, int a, int d, int tm, float4& x, int& v) {
+  const float4 x0 = A.fix_pos[a];
+  if (tm < 0) {
+    x = make_float4(x0.x, x0.y, x0.z, 1.0f);
+    if (!A.pos_only) v = A.fix_v[a];
+    return;
+  }
+  const uint2 key = make_uint2((unsigned)A.seed, (unsigned)(A.seed >> 32));
+  float nz[3];
+  if (A.fix_pos_noise) {
+    const float* pn = A.fix_pos_noise + ((size_t)d * A.n_lig + a) * 3;
+    nz[0] = pn[0]; nz[1] = pn[1]; nz[2] = pn[2];
+  } else {
+    const uint4 r0 = philox4x32_10(make_uint4((unsigned)a, (unsigned)d, 0u, TD_FIX_POS_DOMAIN), key);
+    const float u0 = 1.0f - u01(r0.x), u1 = u01(r0.y), u2 = 1.0f - u01(r0.z), u3 = u01(r0.w);
+    const float ra = sqrtf(-2.0f * logf(u0)), rb = sqrtf(-2.0f * logf(u2));
+    nz[0] = ra * cospif(2.0f * u1); nz[1] = ra * sinpif(2.0f * u1); nz[2] = rb * cospif(2.0f * u3);
+  }
+  const float acv = A.ac[tm];
+  const float sa = sqrtf(acv), sb = sqrtf(1.0f - acv);
+  x.x = __fadd_rn(__fmul_rn(sa, x0.x), __fmul_rn(sb, nz[0]));
+  x.y = __fadd_rn(__fmul_rn(sa, x0.y), __fmul_rn(sb, nz[1]));
+  x.z = __fadd_rn(__fmul_rn(sa, x0.z), __fmul_rn(sb, nz[2]));
+  x.w = 1.0f;
+  if (A.pos_only) return;
+  const int K = A.n_classes, v0 = A.fix_v[a];
+  const float lca = A.lca_v[tm], l1mca = A.l1mca_v[tm] - A.log_k;
+  const float log_eps = -69.07755279f;                                     // logf(1e-30f): index_to_log_onehot's clamp
+  float best = -INFINITY;
+  int vbest = 0;
+  for (int c0 = 0; c0 < K; c0 += 4) {
+    float u[4];
+    if (A.fix_v_uniform) {
+      const float* vu = A.fix_v_uniform + ((size_t)d * A.n_lig + a) * K;
+      for (int j = 0; j < 4 && c0 + j < K; ++j) u[j] = vu[c0 + j];
+    } else {
+      const uint4 r = philox4x32_10(make_uint4((unsigned)a, (unsigned)d, 1u + (unsigned)(c0 >> 2), TD_FIX_TYPE_DOMAIN), key);
+      u[0] = u01(r.x); u[1] = u01(r.y); u[2] = u01(r.z); u[3] = u01(r.w);
+    }
+    for (int j = 0; j < 4 && c0 + j < K; ++j) {
+      const int c = c0 + j;
+      const float lp = log_add_exp_f(((c == v0) ? 0.0f : log_eps) + lca, l1mca);
+      const float sc = -logf(-logf(u[j] + 1e-30f) + 1e-30f) + lp;
+      if (sc > best) { best = sc; vbest = c; }
+    }
+  }
+  v = vbest;
+}
+
+// kFixed = false (no fixed set) compiles to the step as it was before fixed atoms existed
+template <bool kFixed>
 __global__ void step_epilogue_kernel(TdStepArgs A) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a >= A.n_lig) return;
   const int s = *A.step;                       // steps done so far
   const int t = A.t_start - s;                 // current timestep (reference :649-651)
   const int K = A.n_classes;
+  const bool fixed = kFixed && A.fix_mask[a];
 
   // noise for this atom
   float nz[3];
@@ -82,6 +143,9 @@ __global__ void step_epilogue_kernel(TdStepArgs A) {
   xn.y = (c0 * x0.y + ct * xt.y) + sig * nz[1];
   xn.z = (c0 * x0.z + ct * xt.z) + sig * nz[2];
   xn.w = 1.0f;
+  // a fixed row is overwritten after the update: q(x_{t-1} | x0_f) from draw s + 1, or x0_f itself after t = 0
+  int vfix = 0;
+  if (fixed) fixed_sample(A, a, s + 1, t - 1, xn, vfix);
   A.lig_pos[a] = xn;
   const float4 off = A.offset[g];
   if (A.pos_traj) {
@@ -127,6 +191,7 @@ __global__ void step_epilogue_kernel(TdStepArgs A) {
       if (o0) o0[c] = lr[c];
       if (ot) ot[c] = lp;
     }
+    if (fixed) vnew = vfix;                    // v0_traj / vt_traj above keep the model's own opinion of the row
     A.lig_v[a] = vnew;
   }
   if (A.v_traj) A.v_traj[(size_t)s * A.n_lig + a] = (long long)vnew;
@@ -135,8 +200,48 @@ __global__ void step_epilogue_kernel(TdStepArgs A) {
 __global__ void advance_step_kernel(int* step) { *step += 1; }
 
 void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st) {
-  if (A.n_lig > 0) step_epilogue_kernel<<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
+  if (A.n_lig > 0) {
+    if (A.fix_mask) step_epilogue_kernel<true><<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
+    else step_epilogue_kernel<false><<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
+  }
   advance_step_kernel<<<1, 1, 0, st>>>(A.step);
+}
+
+// fixed rows <- q(x_{T-1} | x0_f), q(v_{T-1} | v0_f) from draw 0, once before the first step of a chain
+__global__ void fixed_init_kernel(TdStepArgs A) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= A.n_lig || !A.fix_mask[a]) return;
+  float4 x;
+  int v = A.lig_v[a];
+  fixed_sample(A, a, 0, A.t_start, x, v);
+  A.lig_pos[a] = x;
+  A.lig_v[a] = v;
+}
+void td_launch_fixed_init(const TdStepArgs& A, cudaStream_t st) {
+  if (A.n_lig > 0) fixed_init_kernel<<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
+}
+
+// fixed set in (tdiff_set_fixed): positions and classes are read at masked rows only; lab frame -> centred like set_ligand_kernel
+__global__ void set_fixed_kernel(const unsigned char* __restrict__ mask, const float* __restrict__ pos, const long long* __restrict__ v,
+                                 const int* __restrict__ lig_graph, const float4* __restrict__ offset, int apply_center, int n, int n_classes,
+                                 unsigned char* __restrict__ fix_mask, float4* __restrict__ fix_pos, int* __restrict__ fix_v, int* __restrict__ err) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= n) return;
+  const unsigned char m = mask[a] ? 1 : 0;
+  fix_mask[a] = m;
+  if (!m) { fix_pos[a] = make_float4(0.f, 0.f, 0.f, 1.0f); fix_v[a] = 0; return; }
+  float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (apply_center) o = offset[lig_graph[a]];
+  fix_pos[a] = make_float4(pos[3 * a] - o.x, pos[3 * a + 1] - o.y, pos[3 * a + 2] - o.z, 1.0f);
+  const long long vv = v[a];
+  if (vv < 0 || vv >= n_classes) { atomicExch(err, 1); fix_v[a] = 0; }
+  else fix_v[a] = (int)vv;
+}
+void td_launch_set_fixed(const unsigned char* mask, const float* pos, const long long* v, const int* lig_graph, const float4* offset,
+                         int apply_center, int n, int n_classes, unsigned char* fix_mask, float4* fix_pos, int* fix_v, int* err,
+                         cudaStream_t st) {
+  if (n > 0) set_fixed_kernel<<<(n + 255) / 256, 256, 0, st>>>(mask, pos, v, lig_graph, offset, apply_center, n, n_classes, fix_mask, fix_pos,
+                                                               fix_v, err);
 }
 
 // ---------------------------------------------------------------------------------------- state marshalling

@@ -25,9 +25,20 @@ struct TdStepArgs {
   long long* v_traj;               // [S,Nl] or NULL
   float* v0_traj;                  // [S,Nl,K] or NULL
   float* vt_traj;                  // [S,Nl,K] or NULL
+  // fixed atoms (tdiff_set_fixed); fix_mask == NULL: none, and the kernel takes the default path only
+  const unsigned char* fix_mask;   // [Nl] 1 = the row is held to the forward process of (fix_pos, fix_v)
+  const float4* fix_pos;           // [Nl] target positions x0_f, centred frame
+  const int* fix_v;                // [Nl] target classes v0_f
+  const float* ac;                 // alphas_cumprod [T]
+  const float* fix_pos_noise;      // fixed-atom tape [S+1,Nl,3] or NULL (Philox, FIX_POS domain)
+  const float* fix_v_uniform;      // fixed-atom tape [S+1,Nl,K] or NULL (Philox, FIX_TYPE domain)
 };
 
 void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st);
+void td_launch_fixed_init(const TdStepArgs& A, cudaStream_t st);
+void td_launch_set_fixed(const unsigned char* mask, const float* pos, const long long* v, const int* lig_graph, const float4* offset,
+                         int apply_center, int n, int n_classes, unsigned char* fix_mask, float4* fix_pos, int* fix_v, int* err,
+                         cudaStream_t st);
 void td_launch_segment_mean3(const float* pos, const int* seg_ptr, int n_seg, float4* out, cudaStream_t st);
 void td_launch_place_protein(const float* pos, const int* prot_node, const int* prot_graph, const float4* offset, int n, float4* xm0,
                              float4* xm1, cudaStream_t st);

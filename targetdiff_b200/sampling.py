@@ -9,7 +9,15 @@ counter-based Philox stream keyed by a seed drawn from torch's CPU generator (so
 `randn_like(center)` (:63), `rand_like(uniform_logits)` (:69 via models/molopt_score_model.py:161), then per denoising step
 `randn_like(ligand_pos)` and `rand_like(log_model_prob)` (models/molopt_score_model.py:678,685) -- pre-drawn as a noise tape.
 A run seeded with `seed_all(s)` then consumes the same random numbers as the unmodified reference run on CPU with the same
-seed, which is what "identical RNG seeds" parity needs (tests/golden/pocket_1h36_*.npz were produced that way)."""
+seed, which is what "identical RNG seeds" parity needs (tests/golden/pocket_1h36_*.npz were produced that way).
+
+Fragment-conditioned sampling (an extension beyond the reference, DESIGN.md section 1).  `fixed_ligand=(pos [n_f,3] lab frame,
+v [n_f] class indices)` puts the fragment in the first n_f rows of every sample's ligand and holds those atoms to the forward process
+of the fragment through the chain (ScorePosNet3D.sample_diffusion(fixed_mask=...)); they end exactly at `pos` / `v`.  Each sample's
+size comes from `sample_num_atoms` as without a fragment and is raised to n_f + 1 where it is smaller, so that every sample grows at
+least one atom.  The initial draws still cover every row (the fragment rows' values are replaced), so under rng='cpu' the generator
+is consumed as without a fragment, followed by the fixed atoms' tape: randn(S+1, Nl, 3), then rand(S+1, Nl, K).  `pos_only=True`
+keeps the reference ligand's types and cannot take a fragment."""
 import time
 
 import numpy as np
@@ -32,9 +40,21 @@ def _split(arr, cum, n_data):
 
 
 def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cuda:0', num_steps=None, pos_only=False,
-                            center_pos_mode='protein', sample_num_atoms='prior', rng='device'):
+                            center_pos_mode='protein', sample_num_atoms='prior', rng='device', fixed_ligand=None):
     if rng not in ('device', 'cpu'):
         raise ValueError("rng must be 'device' or 'cpu'")
+    n_f = 0
+    if fixed_ligand is not None:
+        if pos_only:
+            raise ValueError('pos_only=True keeps the reference ligand\'s atom types and cannot take a fixed fragment')
+        frag_pos = torch.as_tensor(fixed_ligand[0]).detach().cpu().float()
+        frag_v = torch.as_tensor(fixed_ligand[1]).detach().cpu().long()
+        n_f = frag_v.shape[0]
+        if frag_pos.dim() != 2 or frag_pos.shape != (n_f, 3) or frag_v.dim() != 1 or n_f < 1:
+            raise ValueError('fixed_ligand must be (pos [n_f,3], v [n_f]) with n_f >= 1; got shapes %s, %s'
+                             % (tuple(frag_pos.shape), tuple(frag_v.shape)))
+        if int(frag_v.min()) < 0 or int(frag_v.max()) >= model.num_classes:
+            raise ValueError('fixed_ligand classes must lie in 0..%d' % (model.num_classes - 1))
     all_pred_pos, all_pred_v = [], []
     all_pred_pos_traj, all_pred_v_traj = [], []
     all_pred_v0_traj, all_pred_vt_traj = [], []
@@ -60,6 +80,8 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
                 ligand_num_atoms = [int(data.ligand_element.size(0))] * n_data
             else:
                 raise ValueError
+            if n_f:
+                ligand_num_atoms = [max(n, n_f + 1) for n in ligand_num_atoms]
             batch_ligand = torch.repeat_interleave(torch.arange(n_data), torch.tensor(ligand_num_atoms)).to(device)
             protein_pos = protein_pos_dev.repeat(n_data, 1)
             protein_v = protein_feat_dev.repeat(n_data, 1)
@@ -86,11 +108,23 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
                     if not pos_only:
                         vu[st] = torch.rand(n_lig, model.num_classes)
                 tape = (pn, vu)
+            fixed = {}
+            if n_f:
+                starts = np.cumsum([0] + ligand_num_atoms[:-1])
+                rows = torch.from_numpy((starts[:, None] + np.arange(n_f)[None, :]).reshape(-1)).to(device)
+                mask = torch.zeros(n_lig, dtype=torch.bool, device=device)
+                mask[rows] = True
+                init_ligand_pos[rows] = frag_pos.to(device).repeat(n_data, 1)
+                init_ligand_v = init_ligand_v.clone()
+                init_ligand_v[rows] = frag_v.to(device).repeat(n_data)
+                fixed['fixed_mask'] = mask
+                if rng == 'cpu':
+                    fixed['fixed_noise_tape'] = (torch.randn(S + 1, n_lig, 3), torch.rand(S + 1, n_lig, model.num_classes))
 
             r = model.sample_diffusion(protein_pos=protein_pos, protein_v=protein_v, batch_protein=batch_protein,
                                        init_ligand_pos=init_ligand_pos, init_ligand_v=init_ligand_v, batch_ligand=batch_ligand,
                                        num_steps=num_steps, pos_only=pos_only, center_pos_mode=center_pos_mode, stack_traj=True,
-                                       noise_tape=tape)
+                                       noise_tape=tape, **fixed)
             cum = np.cumsum([0] + ligand_num_atoms)
             pos = r['pos'].cpu().numpy().astype(np.float64)
             all_pred_pos += [pos[cum[k]:cum[k + 1]] for k in range(n_data)]

@@ -358,14 +358,19 @@ class ScorePosNet3D(nn.Module):
     @torch.no_grad()
     def sample_diffusion(self, protein_pos, protein_v, batch_protein, init_ligand_pos, init_ligand_v, batch_ligand,
                          num_steps=None, center_pos_mode=None, pos_only=False, noise_tape=None, seed=None, return_traj=True,
-                         stack_traj=False):
+                         stack_traj=False, fixed_mask=None, fixed_noise_tape=None):
         """The reverse-diffusion chain (reference models/molopt_score_model.py:633-703), executed entirely by libtdiff.so.
 
         Extensions over the reference signature (all optional): `noise_tape=(pos_noise [S,Nl,3], v_uniform [S,Nl,K])`
         replaces the RNG in the reference's draw order (parity tests); `seed` keys the device Philox generator (default:
         drawn from torch's global CPU generator, so `seed_all` makes runs reproducible); `return_traj=False` skips the
         four trajectory outputs; `stack_traj=True` returns each trajectory as one stacked CPU tensor [S, ...] instead
-        of the reference's list of per-step tensors."""
+        of the reference's list of per-step tensors.
+
+        Fixed atoms (fragment-conditioned sampling, DESIGN.md section 1): `fixed_mask` [Nl] bool holds the masked ligand atoms to the
+        forward process of their `init_ligand_pos` / `init_ligand_v` rows (lab frame) through the chain; they end exactly there.
+        `fixed_noise_tape=(pos_noise [S+1,Nl,3], v_uniform [S+1,Nl,K])` replaces their draws; it is required with `noise_tape` and
+        not allowed without it.  pos_traj / v_traj show the fixed rows as held, v0_traj / vt_traj what the network made of them."""
         if num_steps is None:
             num_steps = self.num_timesteps
         mode = {None: 0, 'none': 0, 'protein': 1}.get(center_pos_mode, None)
@@ -386,6 +391,23 @@ class ScorePosNet3D(nn.Module):
             v_uniform = noise_tape[1].detach().to(dev, torch.float32).contiguous()
             if tuple(pos_noise.shape) != (S, Nl, 3) or tuple(v_uniform.shape) != (S, Nl, K):
                 raise ValueError('noise tape shapes must be [S,Nl,3] and [S,Nl,K]')
+        fix_pn = fix_vu = None
+        if fixed_mask is not None:
+            mask = torch.as_tensor(fixed_mask).detach().to(dev, torch.uint8).contiguous()
+            if tuple(mask.shape) != (Nl,):
+                raise ValueError('fixed_mask must have one entry per ligand atom: shape %s, %d atoms' % (tuple(mask.shape), Nl))
+            if fixed_noise_tape is not None:
+                fix_pn = fixed_noise_tape[0].detach().to(dev, torch.float32).contiguous()
+                if tuple(fix_pn.shape) != (S + 1, Nl, 3):
+                    raise ValueError('fixed noise tape positions must be [S+1,Nl,3] = %s, got %s' % ((S + 1, Nl, 3), tuple(fix_pn.shape)))
+                if not pos_only:
+                    fix_vu = fixed_noise_tape[1].detach().to(dev, torch.float32).contiguous()
+                    if tuple(fix_vu.shape) != (S + 1, Nl, K):
+                        raise ValueError('fixed noise tape uniforms must be [S+1,Nl,K] = %s, got %s' % ((S + 1, Nl, K), tuple(fix_vu.shape)))
+            _lib.check(lib.tdiff_set_fixed(eng, _ptr(mask), _ptr(lpos), _ptr(lv), mode, st))
+            _lib.check(lib.tdiff_set_fixed_tape(eng, _ptr(fix_pn), _ptr(fix_vu)))
+        elif fixed_noise_tape is not None:
+            raise ValueError('fixed_noise_tape without fixed_mask')
         if seed is None:        # with a tape the Philox key is unused: do not advance the caller's CPU generator (rng='cpu' driver parity)
             seed = 0 if noise_tape is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
         pos_traj = v_traj = v0_traj = vt_traj = None
