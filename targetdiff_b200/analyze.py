@@ -11,10 +11,17 @@ from . import _lib
 
 def check_stability_batch(positions, atom_types, hs=False, device='cuda:0'):
     """positions: list of [n_i,3] arrays (or one [sum n_i,3] tensor with `atom_types` a list of arrays); atom_types: atomic numbers.
+    Every coordinate must be an fp32 value (the sampler's positions, fp32 widened to float64, are): the screen computes in float64
+    on exactly those values, as the reference does, and refuses others with ValueError rather than rounding them.
     Returns (molecule_stable [M] bool, nr_stable_atoms [M] int, n_atoms [M] int, nr_bonds [sum n_i] int) as numpy arrays."""
     counts = [len(a) for a in atom_types]
-    pos = torch.as_tensor(np.concatenate([np.asarray(p, dtype=np.float64) for p in positions]) if isinstance(positions, (list, tuple))
-                          else np.asarray(positions)).to(torch.float32)
+    as64 = lambda p: np.asarray(p, dtype=np.float64).reshape(0, 3) if np.size(p) == 0 else np.asarray(p, dtype=np.float64)   # zero atoms
+    pos64 = np.concatenate([as64(p) for p in positions]) if isinstance(positions, (list, tuple)) else np.asarray(positions, dtype=np.float64)
+    pos = torch.from_numpy(pos64.astype(np.float32))
+    if not np.array_equal(pos.numpy().astype(np.float64), pos64, equal_nan=True):
+        # the kernel reads fp32 coordinates: rounding others would screen different atoms from the ones the reference would
+        raise ValueError('positions must be fp32 values (as the sampler returns them, widened or not): %d coordinates are not'
+                         % int((pos.numpy().astype(np.float64) != pos64).sum()))
     z = torch.as_tensor(np.concatenate([np.asarray(a).astype(np.int64) for a in atom_types])).to(torch.int32)
     if pos.shape[0] != sum(counts) or pos.dim() != 2 or pos.shape[1] != 3:
         raise ValueError('positions must be [n,3] per molecule')

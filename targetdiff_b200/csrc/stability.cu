@@ -4,8 +4,10 @@
 // generated molecule by scripts/evaluate_diffusion.py:78-84) and its helper `get_bond_order` (:90-103): for every atom pair the
 // distance in picometres is compared with the single / double / triple bond-length tables (+ margins 10 / 5 / 3 pm), the bond orders
 // are summed per atom, and an atom is stable when 0 < bonds <= its allowed valence (== with `hs`).
-// One warp per molecule; arithmetic in fp64 exactly as numpy does on the float64 positions the sampler returns
-// (difference, square, ((a + b) + c), sqrt, * 100), so no comparison can flip against the reference.
+// One warp per molecule; arithmetic in fp64 rounded op by op as numpy does on the float64 positions the sampler returns (fp32 values):
+// difference, each square, ((a + b) + c), sqrt, * 100.  The squared distance is written with __dmul_rn / __dadd_rn, which nvcc never
+// contracts: with plain operators it fuses two of the products into DFMAs, and pairs within an ulp of a threshold then get another
+// bond order than the reference's (DESIGN.md section 2, stability screen).  Double sqrt and the product are correctly rounded.
 #include "tdiff_common.cuh"
 
 namespace {
@@ -49,7 +51,7 @@ check_stability_kernel(const float* __restrict__ pos, const int* __restrict__ at
       // the reference always evaluates the pair with the smaller index first: p1 - p2 and bonds[atom1][atom2] of (min, max); the tables
       // are symmetric and (-d)^2 == d^2, so the order does not matter
       const double dx = xi - (double)pos[3 * (b + j)], dy = yi - (double)pos[3 * (b + j) + 1], dz = zi - (double)pos[3 * (b + j) + 2];
-      const double dist = 100.0 * sqrt((dx * dx + dy * dy) + dz * dz);                       // analyze.py:91,119
+      const double dist = 100.0 * sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));  // analyze.py:91,119
       int order = 0;
       if (dist < (double)(c_bonds1[ei][ej] + 10)) {                                          // margin1
         order = 1;
