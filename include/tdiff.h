@@ -165,6 +165,29 @@ TDIFF_API int tdiff_set_fixed(tdiff_engine* e, const uint8_t* d_mask, const floa
                               void* stream);
 TDIFF_API int tdiff_set_fixed_tape(tdiff_engine* e, const float* d_pos_noise, const float* d_v_uniform);
 
+/* Respaced sampling (an extension beyond the reference, DESIGN.md section 1): the chain of tdiff_sample on a time sequence
+ * h_time_seq[0..S-1] (host memory, S = num_steps), integers tau_0 > tau_1 > ... > tau_{S-1} >= 0 with tau_0 = T - 1 and 1 <= S <= T.
+ * Step s evaluates the network at t = tau_s, exactly as tdiff_sample does at t, and moves the state to time p = tau_{s+1}, or to
+ * p = tau_{S-1} - 1 at the last step (the decoder step, sigma = 0, when tau_{S-1} = 0: a sequence that ends at 0 finishes the molecule).
+ *   Unit steps (p = t - 1) use the checkpoint's tables at t, so T-1, ..., 0 is tdiff_sample(T) and T-1, ..., T-S is tdiff_sample(S),
+ *   bit for bit.
+ *   Jump steps (p < t - 1) use the exact posteriors q(x_p | x_t, x0), q(v_p | v_t, v0).  With abar = alphas_cumprod, a = abar_t / abar_p:
+ *     x_p = c0 x0 + ct x_t + sigma eps, c0 = sqrt(abar_p) (1 - a) / (1 - abar_t), ct = sqrt(a) (1 - abar_p) / (1 - abar_t),
+ *     sigma^2 = (1 - abar_p) (1 - a) / (1 - abar_t);
+ *     log q(v_p | v_t, v0) = normalise[log_add_exp(log v0 + lcabar_v[p], l1mcabar_v[p] - log K)
+ *                                      + log_add_exp(log v_t + lambda, log(1 - e^lambda + 1e-40) - log K)],
+ *     lambda = sum_{i = p+1..t} log_alphas_v[i].
+ *   The host computes these in double from the fp32 'betas' (1 - abar = -expm1(sum log1p(-beta))) and 'log_alphas_v' tables and
+ *   rounds each to fp32 once; the tables are uploaded before the chain (one stream synchronisation).
+ * Everything else is tdiff_sample's: tapes [S,Nl,...] and Philox counters keyed by the step index s, trajectories [S,...] (entry s is
+ * the state after step s, at time p), the same launches per step, one captured graph.  Fixed atoms (tdiff_set_fixed): after step s
+ * the fixed rows get a sample at p from draw s + 1 (the fixed tape is [S+1,Nl,...]), or x0_f / v0_f after the step at tau_{S-1} = 0.
+ * A time embedding sees tau_s / T.  A NULL, empty, too long, not strictly decreasing or negative sequence, or one not starting at
+ * T - 1 -> TDIFF_EINVAL. */
+TDIFF_API int tdiff_sample_seq(tdiff_engine* e, const int32_t* h_time_seq, int num_steps, const float* d_pos_noise, const float* d_v_uniform,
+                               uint64_t seed, float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only,
+                               void* stream);
+
 /* Same loop through HOST buffers (the end-to-end path: H2D of the inputs, the chain, D2H of the results, all on
  * `stream`, synchronised before returning).  Equivalent of the device-facing part of sample_diffusion_ligand
  * (scripts/sample_diffusion.py:42-112) for one batch.  h_out_* may be NULL. */

@@ -14,7 +14,9 @@
 
 Result file: `<result_path>/sample.pt` (sample_for_pocket) or `<result_path>/result_{i}.pt` (sample_pockets) = {'data', 'pred_ligand_pos', 'pred_ligand_v', 'pred_ligand_pos_traj', 'pred_ligand_v_traj', 'time'}
 -- the schema scripts/sample_diffusion.py:175-182 writes and scripts/evaluate_diffusion.py:70-76 reads (positions float64, per-sample
-lists; trajectories [steps, atoms, 3]).  Molecule reconstruction / SDF writing needs RDKit + OpenBabel and stays out of scope."""
+lists; trajectories [steps, atoms, 3]).  With `sample.respaced_steps: n` in the config (an extension beyond the reference) both commands
+run the n-step chain of sampling.respaced_time_seq(T, n) instead of num_steps, and the result also holds 'time_seq'.  Molecule
+reconstruction / SDF writing needs RDKit + OpenBabel and stays out of scope."""
 import argparse
 import os
 import shutil
@@ -22,7 +24,7 @@ import sys
 
 import torch
 
-from .config import load_config
+from .config import load_config, sampling_time_seq
 from .pocket import pdb_to_pocket_data
 from .sampling import sample_diffusion_ligand, seed_all
 from .score_model import ScorePosNet3D
@@ -59,6 +61,13 @@ def _load_model(config, device, rank=0):
     model = model.to(device)
     tdist.broadcast_state_dict(model, src=0)
     return model
+
+
+def _time_seq(config, model):
+    """The time sequence `sample.respaced_steps` asks for (config.sampling_time_seq), or None for the default chain."""
+    if config.sample.get('respaced_steps') is None:
+        return None
+    return sampling_time_seq(config.sample, model.num_timesteps)
 
 
 def list_pockets(pocket_dir=None, pocket_list=None):
@@ -116,6 +125,8 @@ def sample_pockets(argv):
     paths = list_pockets(a.pocket_dir, a.pocket_list)
     mine = assign_pockets(paths, rank, world, a.schedule, a.data_id)
     model = _load_model(config, device, rank)
+    time_seq = _time_seq(config, model)
+    num_steps = config.sample.num_steps if time_seq is None else None
     n = a.num_samples if a.num_samples is not None else config.sample.num_samples
     os.makedirs(a.result_path, exist_ok=True)
     if rank == 0:
@@ -124,10 +135,13 @@ def sample_pockets(argv):
     for i in mine:
         seed_all(config.sample.seed)          # the reference starts one process per pocket, each seeded the same way (:133)
         data = pdb_to_pocket_data(paths[i])
-        outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=device, num_steps=config.sample.num_steps,
+        outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=device, num_steps=num_steps,
                                           pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
-                                          sample_num_atoms=config.sample.sample_num_atoms)
-        torch.save(build_result(data, outputs), os.path.join(a.result_path, 'result_%d.pt' % i))
+                                          sample_num_atoms=config.sample.sample_num_atoms, time_seq=time_seq)
+        result = build_result(data, outputs)
+        if time_seq is not None:
+            result['time_seq'] = time_seq
+        torch.save(result, os.path.join(a.result_path, 'result_%d.pt' % i))
         done.append((i, len(outputs[0]), sum(outputs[-1])))
         print('[rank %d/%d] pocket %d (%s): %d molecules, %.1f s' % (rank, world, i, os.path.basename(paths[i]), done[-1][1], done[-1][2]))
     return done
@@ -167,16 +181,20 @@ def sample_for_pocket(argv):
     fragment = load_fragment(a.fragment) if a.fragment else None
     seed_all(config.sample.seed)
     model = _load_model(config, a.device)
+    time_seq = _time_seq(config, model)
     data = pdb_to_pocket_data(a.pdb_path)
     n = a.num_samples if a.num_samples is not None else config.sample.num_samples
-    outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=a.device, num_steps=config.sample.num_steps,
-                                      pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
-                                      sample_num_atoms=config.sample.sample_num_atoms, fixed_ligand=fragment)
+    outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=a.device,
+                                      num_steps=config.sample.num_steps if time_seq is None else None, pos_only=config.sample.pos_only,
+                                      center_pos_mode=config.sample.center_pos_mode, sample_num_atoms=config.sample.sample_num_atoms,
+                                      fixed_ligand=fragment, time_seq=time_seq)
     os.makedirs(a.result_path, exist_ok=True)
     shutil.copyfile(a.config, os.path.join(a.result_path, 'sample.yml'))
     result = build_result(data, outputs)
     if fragment is not None:
         result['fixed_ligand_atoms'] = int(fragment[1].shape[0])
+    if time_seq is not None:
+        result['time_seq'] = time_seq
     torch.save(result, os.path.join(a.result_path, 'sample.pt'))
     print('Sample done! %d molecules, %.1f s' % (len(outputs[0]), sum(outputs[-1])))
 

@@ -46,6 +46,21 @@ def default_sampling_config():
                                 sample_num_atoms='prior'))
 
 
+def sampling_time_seq(sample, T):
+    """The time sequence `sample.respaced_steps` = n asks for (sampling.respaced_time_seq(T, n), an extension beyond the reference's
+    sampling.yml), or None for the default chain.  ValueError when it is given with a `sample.num_steps` other than T: the two would
+    ask for different chains."""
+    n = sample.get('respaced_steps')
+    if n is None:
+        return None
+    steps = sample.get('num_steps', T)
+    if steps is not None and int(steps) != T:
+        raise ValueError('sample.respaced_steps=%s cannot be combined with sample.num_steps=%s (num_steps truncates the chain; '
+                         'leave it at T = %d)' % (n, steps, T))
+    from .sampling import respaced_time_seq
+    return respaced_time_seq(T, n)
+
+
 # Values the sm_90a engine implements; anything else is rejected loudly (SURVEY.md 8(b) "should-reject-clearly").
 _SUPPORTED = dict(model_mean_type=('C0', 'noise'), beta_schedule=('sigmoid', 'linear', 'quad', 'const', 'jsd', 'cosine'),
                   v_beta_schedule=('cosine',), node_indicator=(True,), model_type=('uni_o2',),

@@ -124,6 +124,10 @@ struct tdiff_engine {
   bool has_fixed = false;
   DevBuf fix_mask, fix_pos, fix_v;
   const float *fix_pos_noise = nullptr, *fix_v_uniform = nullptr;
+  // respaced chains (tdiff_sample_seq): double prefix sums over i = 0..t of log(1 - betas[i]) (= log alphas_cumprod[t]) and of
+  // log_alphas_v[i]; the per-step tables of the current chain: seq_t, seq_p [S] int | c0, ct, logvar, la, l1ma [S] fp32
+  std::vector<double> cum_log_a, cum_log_av;
+  DevBuf seq_buf;
   DevBuf stage[8];   // staging for tdiff_sample_host
   // ---- instrumentation
   cudaStream_t own_stream = nullptr;   // capture stream (the caller's stream may be the legacy default stream, which cannot capture)
@@ -451,6 +455,15 @@ extern "C" int tdiff_create(const tdiff_config* cfg, const tdiff_tensor* sd, int
     t.off = pk.alloc(T);
     if (p) memcpy(&pk.host[t.off], p, T * sizeof(float));
   }
+  const float *betas = pk.get("betas", T), *la_v = pk.get("log_alphas_v", T);
+  if (betas && la_v) {           // (a missing table fails tdiff_create below)
+    e->cum_log_a.resize(T); e->cum_log_av.resize(T);
+    double sa = 0.0, sv = 0.0;
+    for (int i = 0; i < T; ++i) {
+      sa += log1p(-(double)betas[i]); e->cum_log_a[i] = sa;
+      sv += (double)la_v[i]; e->cum_log_av[i] = sv;
+    }
+  }
   // embeddings
   const float* wp = pk.get("protein_atom_emb.weight", (int64_t)(TD_H - 1) * F);
   const float* bp = pk.get("protein_atom_emb.bias", TD_H - 1);
@@ -604,7 +617,7 @@ extern "C" void tdiff_destroy(tdiff_engine* e) {
   if (e->ev_join) cudaEventDestroy(e->ev_join);
   DevBuf* bufs[] = {&e->node_ptr, &e->prot_ptr, &e->prot_node, &e->prot_graph, &e->lig_node, &e->lig_graph, &e->node_lig, &e->xm0, &e->xm1,
                     &e->rel_flag, &e->rel_list, &e->n_rel, &e->work_list, &e->n_work, &e->knn_cache, &e->x2h_rows, &e->lig_rows, &e->rel_rows, &e->rel_counts, &e->ew_x2h, &e->ew_h2x, &e->h_sync, &e->hagg, &e->time_norm, &e->h_free, &e->dirty, &e->free_rows, &e->free_counts, &e->lig_save, &e->offset, &e->h0, &e->h, &e->P, &e->q, &e->src, &e->src_prev, &e->etype, &e->e_w, &e->dist, &e->kbuf, &e->vbuf, &e->v16, &e->lig_pos,
-                    &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges, &e->fix_mask, &e->fix_pos, &e->fix_v};
+                    &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges, &e->fix_mask, &e->fix_pos, &e->fix_v, &e->seq_buf};
   for (auto* b : bufs) b->release();
   for (auto& b : e->stage) b.release();
   if (e->arena) cudaFree(e->arena);
@@ -1164,8 +1177,9 @@ void build_free_cache(tdiff_engine* e, cudaStream_t st) {
 }
 
 void run_step(tdiff_engine* e, cudaStream_t st, const TdStepArgs& base) {
-  if (e->time_emb) {               // every graph is at time step t_start - step (reference models/molopt_score_model.py:651)
-    td_launch_set_time(base.step, base.t_start, e->cfg.num_timesteps, e->B, e->time_norm.as<float>(), st);
+  if (e->time_emb) {               // every graph is at time step t_start - step (reference models/molopt_score_model.py:651), or seq_t[step]
+    if (base.seq_t) td_launch_set_time_seq(base.step, base.seq_t, e->cfg.num_timesteps, e->B, e->time_norm.as<float>(), st);
+    else td_launch_set_time(base.step, base.t_start, e->cfg.num_timesteps, e->B, e->time_norm.as<float>(), st);
     e->launches += 1;
   }
   e->restrict_last = true;
@@ -1176,13 +1190,52 @@ void run_step(tdiff_engine* e, cudaStream_t st, const TdStepArgs& base) {
   td_launch_step_epilogue(A, st);
   e->launches += 2;
 }
-}  // namespace
+// Per-step tables of the respaced chain `seq` [S] (DESIGN.md section 1), laid out as e->seq_buf: seq_t, seq_p [S] int32, then c0, ct,
+// logvar, la, l1ma [S] fp32.  Step s moves from t = seq[s] to p = seq[s + 1], or to seq[S - 1] - 1 at the last step.  A unit step
+// (p = t - 1) takes the checkpoint's tables at t.  A jump step takes the exact posterior of the jump t -> p, computed in double from
+// the prefix sums and rounded to fp32 once: with log abar from sum(log1p(-beta)) (never from fp32 alphas_cumprod, whose 1 - abar
+// keeps almost no bits near t = 0) and a = abar_t / abar_p,
+//   c0 = sqrt(abar_p) (1 - a) / (1 - abar_t),  ct = sqrt(a) (1 - abar_p) / (1 - abar_t),  var = (1 - abar_p) (1 - a) / (1 - abar_t),
+//   lambda = sum_{i = p+1..t} log_alphas_v[i],  l1ma = log(1 - e^lambda + 1e-40)   (oracle/respaced.py:jump_tables).
+void seq_tables(const tdiff_engine* e, const int32_t* seq, int S, std::vector<int>& it, std::vector<float>& ft) {
+  const float* H = e->host_arena.data();
+  auto tab = [&](const float* dev, int t) { return H[(dev - e->arena) + t]; };
+  it.assign(2 * (size_t)S, 0);
+  ft.assign(5 * (size_t)S, 0.0f);
+  for (int s = 0; s < S; ++s) {
+    const int t = seq[s], p = s + 1 < S ? seq[s + 1] : t - 1;
+    it[s] = t; it[S + s] = p;
+    float* f = ft.data() + s;
+    if (p == t - 1) {
+      f[0] = tab(e->t_c0, t); f[S] = tab(e->t_ct, t); f[2 * S] = tab(e->t_logvar, t); f[3 * S] = tab(e->t_la, t); f[4 * S] = tab(e->t_l1ma, t);
+      continue;
+    }
+    const double lt = e->cum_log_a[t], lp = e->cum_log_a[p];
+    const double om_t = -expm1(lt), om_p = -expm1(lp), om_a = -expm1(lt - lp);
+    const double lam = e->cum_log_av[t] - e->cum_log_av[p];
+    f[0] = (float)(sqrt(exp(lp)) * om_a / om_t);
+    f[S] = (float)(sqrt(exp(lt - lp)) * om_p / om_t);
+    f[2 * S] = (float)log(om_p * om_a / om_t);
+    f[3 * S] = (float)lam;
+    f[4 * S] = (float)log(1.0 - exp(lam) + 1e-40);
+  }
+}
 
-extern "C" int tdiff_sample(tdiff_engine* e, int num_steps, const float* d_pos_noise, const float* d_v_uniform, uint64_t seed,
-                            float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only, void* stream) {
+// The chain of tdiff_sample (time_seq == NULL) and tdiff_sample_seq: eager first step, then one captured step graph replayed.
+int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const float* d_pos_noise, const float* d_v_uniform, uint64_t seed,
+                 float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only, void* stream) {
   if (!e || !e->bound || !e->has_ligand) return set_err(TDIFF_ESTATE, "sample needs bind_batch + set_ligand first");
   const int T = e->cfg.num_timesteps;
   if (num_steps < 0 || num_steps > T) return set_err(TDIFF_EINVAL, "num_steps=%d outside 0..%d", num_steps, T);
+  if (time_seq) {
+    if (num_steps < 1) return set_err(TDIFF_EINVAL, "time sequence: empty (num_steps=%d)", num_steps);
+    if (time_seq[0] != T - 1) return set_err(TDIFF_EINVAL, "time sequence: starts at %d, not at T - 1 = %d", time_seq[0], T - 1);
+    for (int s = 1; s < num_steps; ++s) {
+      if (time_seq[s] >= time_seq[s - 1])
+        return set_err(TDIFF_EINVAL, "time sequence: not strictly decreasing at step %d (%d after %d)", s, time_seq[s], time_seq[s - 1]);
+      if (time_seq[s] < 0) return set_err(TDIFF_EINVAL, "time sequence: negative time %d at step %d", time_seq[s], s);
+    }
+  }
   if ((d_pos_noise == nullptr) != (d_v_uniform == nullptr) && !pos_only)
     return set_err(TDIFF_EINVAL, "noise tape needs both pos_noise and v_uniform (or neither for Philox)");
   if (e->has_fixed) {      // one noise source per chain: both tapes or neither
@@ -1209,6 +1262,19 @@ extern "C" int tdiff_sample(tdiff_engine* e, int num_steps, const float* d_pos_n
   if (e->has_fixed) {
     A.fix_mask = e->fix_mask.as<unsigned char>(); A.fix_pos = e->fix_pos.as<float4>(); A.fix_v = e->fix_v.as<int>(); A.ac = e->t_ac;
     A.fix_pos_noise = e->fix_pos_noise; A.fix_v_uniform = e->fix_v_uniform;
+  }
+  if (time_seq) {
+    std::vector<int> it;
+    std::vector<float> ft;
+    seq_tables(e, time_seq, num_steps, it, ft);
+    const size_t S = (size_t)num_steps;
+    if (e->seq_buf.ensure(S * 28)) return set_err(TDIFF_ECUDA, "out of device memory for the tables of a %d-step time sequence", num_steps);
+    CK(cudaMemcpyAsync(e->seq_buf.p, it.data(), S * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(e->seq_buf.as<char>() + S * 8, ft.data(), S * 20, cudaMemcpyHostToDevice, st));
+    const int* si = e->seq_buf.as<int>();
+    const float* sf = (const float*)(si + 2 * S);
+    A.seq_t = si; A.seq_p = si + S;
+    A.seq_c0 = sf; A.seq_ct = sf + S; A.seq_logvar = sf + 2 * S; A.seq_la = sf + 3 * S; A.seq_l1ma = sf + 4 * S;
   }
   CK(cudaMemsetAsync(e->step.p, 0, sizeof(int), st));
   if (e->has_fixed) {      // the chain's one extra launch: fixed rows <- q(x_{T-1} | x0_f), q(v_{T-1} | v0_f)
@@ -1258,6 +1324,19 @@ extern "C" int tdiff_sample(tdiff_engine* e, int num_steps, const float* d_pos_n
   delete total;
   CK(cudaGetLastError());
   return TDIFF_OK;
+}
+}  // namespace
+
+extern "C" int tdiff_sample(tdiff_engine* e, int num_steps, const float* d_pos_noise, const float* d_v_uniform, uint64_t seed,
+                            float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only, void* stream) {
+  return sample_chain(e, nullptr, num_steps, d_pos_noise, d_v_uniform, seed, d_pos_traj, d_v_traj, d_v0_traj, d_vt_traj, pos_only, stream);
+}
+
+extern "C" int tdiff_sample_seq(tdiff_engine* e, const int32_t* h_time_seq, int num_steps, const float* d_pos_noise, const float* d_v_uniform,
+                                uint64_t seed, float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only,
+                                void* stream) {
+  if (!h_time_seq) return set_err(TDIFF_EINVAL, "time sequence: null pointer");
+  return sample_chain(e, h_time_seq, num_steps, d_pos_noise, d_v_uniform, seed, d_pos_traj, d_v_traj, d_v0_traj, d_vt_traj, pos_only, stream);
 }
 
 extern "C" int tdiff_sample_host(tdiff_engine* e, int B, const int32_t* pc, const int32_t* lc, const float* h_ppos, const float* h_pfeat,

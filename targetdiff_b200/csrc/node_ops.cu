@@ -85,6 +85,15 @@ __global__ void set_time_kernel(const int* __restrict__ step, int t_start, int n
 void td_launch_set_time(const int* step, int t_start, int n_timesteps, int n_graphs, float* time_norm, cudaStream_t st) {
   if (n_graphs > 0) set_time_kernel<<<(n_graphs + 255) / 256, 256, 0, st>>>(step, t_start, n_timesteps, n_graphs, time_norm);
 }
+// respaced chain: every graph is at time step time_seq[step]
+__global__ void set_time_seq_kernel(const int* __restrict__ step, const int* __restrict__ time_seq, int n_timesteps, int n_graphs,
+                                    float* __restrict__ time_norm) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n_graphs) time_norm[g] = (float)time_seq[*step] / (float)n_timesteps;
+}
+void td_launch_set_time_seq(const int* step, const int* time_seq, int n_timesteps, int n_graphs, float* time_norm, cudaStream_t st) {
+  if (n_graphs > 0) set_time_seq_kernel<<<(n_graphs + 255) / 256, 256, 0, st>>>(step, time_seq, n_timesteps, n_graphs, time_norm);
+}
 
 // ---------------------------------------------------------------------------------------------- node projection
 // P[N,640] = h[N,128] . wn_t[128][640] + bn ; CTA tile 128 rows x 128 columns.

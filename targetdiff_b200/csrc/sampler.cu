@@ -86,13 +86,16 @@ __device__ __forceinline__ void fixed_sample(const TdStepArgs& A, int a, int d, 
   v = vbest;
 }
 
-// kFixed = false (no fixed set) compiles to the step as it was before fixed atoms existed
-template <bool kFixed>
+// kFixed = false (no fixed set) compiles to the step as it was before fixed atoms existed.  kSeq = true runs step s of a respaced
+// chain (DESIGN.md section 1): the network saw t = seq_t[s], and the state moves to p = seq_p[s] with the per-step coefficients
+// seq_*[s]; kSeq = false is the default chain t = t_start - s, p = t - 1 on the checkpoint's tables.
+template <bool kFixed, bool kSeq>
 __global__ void step_epilogue_kernel(TdStepArgs A) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a >= A.n_lig) return;
   const int s = *A.step;                       // steps done so far
-  const int t = A.t_start - s;                 // current timestep (reference :649-651)
+  const int t = kSeq ? A.seq_t[s] : A.t_start - s;   // current timestep (reference :649-651)
+  const int p = kSeq ? A.seq_p[s] : t - 1;           // the time this step moves to
   const int K = A.n_classes;
   const bool fixed = kFixed && A.fix_mask[a];
 
@@ -136,16 +139,16 @@ __global__ void step_epilogue_kernel(TdStepArgs A) {
     x0.y = ra * xt.y - rm * (x0.y - xt.y);
     x0.z = ra * xt.z - rm * (x0.z - xt.z);
   }
-  const float c0 = A.c0[t], ct = A.ct[t];
-  const float sig = ((t == 0) ? 0.0f : 1.0f) * expf(0.5f * A.logvar[t]);
+  const float c0 = kSeq ? A.seq_c0[s] : A.c0[t], ct = kSeq ? A.seq_ct[s] : A.ct[t];
+  const float sig = ((t == 0) ? 0.0f : 1.0f) * expf(0.5f * (kSeq ? A.seq_logvar[s] : A.logvar[t]));
   float4 xn;
   xn.x = (c0 * x0.x + ct * xt.x) + sig * nz[0];
   xn.y = (c0 * x0.y + ct * xt.y) + sig * nz[1];
   xn.z = (c0 * x0.z + ct * xt.z) + sig * nz[2];
   xn.w = 1.0f;
-  // a fixed row is overwritten after the update: q(x_{t-1} | x0_f) from draw s + 1, or x0_f itself after t = 0
+  // a fixed row is overwritten after the update: q(x_p | x0_f) from draw s + 1, or x0_f itself after t = 0
   int vfix = 0;
-  if (fixed) fixed_sample(A, a, s + 1, t - 1, xn, vfix);
+  if (fixed) fixed_sample(A, a, s + 1, p, xn, vfix);
   A.lig_pos[a] = xn;
   const float4 off = A.offset[g];
   if (A.pos_traj) {
@@ -164,9 +167,9 @@ __global__ void step_epilogue_kernel(TdStepArgs A) {
     for (int c = 0; c < K; ++c) se += expf(lr[c] - mx);
     const float lse = logf(se);
     for (int c = 0; c < K; ++c) lr[c] = (lr[c] - mx) - lse;                 // log_softmax
-    const int tm1 = t > 0 ? t - 1 : 0;
+    const int tm1 = kSeq ? (p > 0 ? p : 0) : (t > 0 ? t - 1 : 0);
     const float lca = A.lca_v[tm1], l1mca = A.l1mca_v[tm1] - A.log_k;
-    const float la = A.la_v[t], l1ma = A.l1ma_v[t] - A.log_k;
+    const float la = kSeq ? A.seq_la[s] : A.la_v[t], l1ma = (kSeq ? A.seq_l1ma[s] : A.l1ma_v[t]) - A.log_k;
     const int vcur = vnew;
     const float log_eps = -69.07755279f;                                   // logf(1e-30f)
     float un_lp[TD_CMAX];
@@ -201,8 +204,14 @@ __global__ void advance_step_kernel(int* step) { *step += 1; }
 
 void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st) {
   if (A.n_lig > 0) {
-    if (A.fix_mask) step_epilogue_kernel<true><<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
-    else step_epilogue_kernel<false><<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
+    const int grid = (A.n_lig + 127) / 128;
+    if (A.seq_t) {
+      if (A.fix_mask) step_epilogue_kernel<true, true><<<grid, 128, 0, st>>>(A);
+      else step_epilogue_kernel<false, true><<<grid, 128, 0, st>>>(A);
+    } else {
+      if (A.fix_mask) step_epilogue_kernel<true, false><<<grid, 128, 0, st>>>(A);
+      else step_epilogue_kernel<false, false><<<grid, 128, 0, st>>>(A);
+    }
   }
   advance_step_kernel<<<1, 1, 0, st>>>(A.step);
 }

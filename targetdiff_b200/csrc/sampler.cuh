@@ -32,6 +32,11 @@ struct TdStepArgs {
   const float* ac;                 // alphas_cumprod [T]
   const float* fix_pos_noise;      // fixed-atom tape [S+1,Nl,3] or NULL (Philox, FIX_POS domain)
   const float* fix_v_uniform;      // fixed-atom tape [S+1,Nl,K] or NULL (Philox, FIX_TYPE domain)
+  // respaced chain (tdiff_sample_seq); seq_t == NULL: the default chain, t = t_start - step, and the kernel takes that path only
+  const int* seq_t;                // [S] tau_s, the time the network sees at step s
+  const int* seq_p;                // [S] the time step s moves to: tau_{s+1}, or tau_{S-1} - 1 at the last step
+  const float *seq_c0, *seq_ct, *seq_logvar;   // [S] position posterior of the jump t -> p (the checkpoint's tables at t on unit steps)
+  const float *seq_la, *seq_l1ma;  // [S] lambda = log of the type schedule's transition probability p -> t, log(1 - e^lambda + 1e-40)
 };
 
 void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st);

@@ -165,6 +165,7 @@ void td_launch_edge_geom_rows(const float4* xm, const int* src, const unsigned c
                               const float* gate_w, float gate_b, const float* offsets, float coeff, float* gate, cudaStream_t st);
 void td_launch_add_rows(const float* a, const float* b, float* out, long long n_floats, cudaStream_t st);
 void td_launch_set_time(const int* step, int t_start, int n_timesteps, int n_graphs, float* time_norm, cudaStream_t st);
+void td_launch_set_time_seq(const int* step, const int* time_seq, int n_timesteps, int n_graphs, float* time_norm, cudaStream_t st);
 void td_launch_edge_mlp_tc(const float* P, const float4* xm, const int* src, const unsigned char* etype, const float* dist,
                            const int* row_nodes, long long n_rows, int k, TdMlp m, const unsigned char* w2_image, int pieces, const float* offsets, float coeff,
                            float* out, int sm_count, cudaStream_t st);

@@ -17,14 +17,19 @@ of the fragment through the chain (ScorePosNet3D.sample_diffusion(fixed_mask=...
 size comes from `sample_num_atoms` as without a fragment and is raised to n_f + 1 where it is smaller, so that every sample grows at
 least one atom.  The initial draws still cover every row (the fragment rows' values are replaced), so under rng='cpu' the generator
 is consumed as without a fragment, followed by the fixed atoms' tape: randn(S+1, Nl, 3), then rand(S+1, Nl, K).  `pos_only=True`
-keeps the reference ligand's types and cannot take a fragment."""
+keeps the reference ligand's types and cannot take a fragment.
+
+Respaced sampling (an extension beyond the reference, DESIGN.md section 1).  `time_seq` (e.g. `respaced_time_seq(T, 100)`) runs the
+chain on that decreasing subsequence of timesteps with the exact jump posteriors (ScorePosNet3D.sample_diffusion(time_seq=...)).
+Under rng='cpu' the tape has S = len(time_seq) steps in the reference's interleaved order, then comes the fixed tape [S+1, ...].
+Whether a checkpoint's molecules keep their quality at fewer steps has not been measured."""
 import time
 
 import numpy as np
 import torch
 
 from . import atom_num
-from .score_model import log_sample_categorical
+from .score_model import check_time_seq, log_sample_categorical
 
 
 def seed_all(seed):
@@ -35,14 +40,29 @@ def seed_all(seed):
     random.seed(seed)
 
 
+def respaced_time_seq(T, n):
+    """n timesteps spaced evenly from T - 1 down to 0, each rounded to the nearest integer (half to even): a strictly decreasing
+    time sequence for ScorePosNet3D.sample_diffusion(time_seq=...).  n = T gives the default chain T-1, ..., 0."""
+    T, n = int(T), int(n)
+    if not 2 <= n <= T:
+        raise ValueError('respaced steps must lie in 2..T = %d, got %d' % (T, n))
+    seq = [int(x) for x in np.rint(np.linspace(T - 1, 0, n))]
+    assert seq[0] == T - 1 and seq[-1] == 0 and all(b < a for a, b in zip(seq, seq[1:]))
+    return seq
+
+
 def _split(arr, cum, n_data):
     return [arr[..., cum[k]:cum[k + 1], :] if arr.ndim == 3 else arr[..., cum[k]:cum[k + 1]] for k in range(n_data)]
 
 
 def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cuda:0', num_steps=None, pos_only=False,
-                            center_pos_mode='protein', sample_num_atoms='prior', rng='device', fixed_ligand=None):
+                            center_pos_mode='protein', sample_num_atoms='prior', rng='device', fixed_ligand=None, time_seq=None):
     if rng not in ('device', 'cpu'):
         raise ValueError("rng must be 'device' or 'cpu'")
+    if time_seq is not None:
+        time_seq = check_time_seq(time_seq, model.num_timesteps)
+        if num_steps is not None and int(num_steps) != len(time_seq):
+            raise ValueError('num_steps=%d disagrees with a time_seq of %d steps' % (int(num_steps), len(time_seq)))
     n_f = 0
     if fixed_ligand is not None:
         if pos_only:
@@ -100,7 +120,7 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
                 init_ligand_v = log_sample_categorical(uniform_logits).to(device)
             tape = None
             if rng == 'cpu':
-                S = model.num_timesteps if num_steps is None else int(num_steps)
+                S = len(time_seq) if time_seq is not None else model.num_timesteps if num_steps is None else int(num_steps)
                 pn = torch.empty(S, n_lig, 3)
                 vu = torch.zeros(S, n_lig, model.num_classes)
                 for st in range(S):                                     # the reference's interleaved draw order
@@ -108,7 +128,7 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
                     if not pos_only:
                         vu[st] = torch.rand(n_lig, model.num_classes)
                 tape = (pn, vu)
-            fixed = {}
+            extra = {} if time_seq is None else {'time_seq': time_seq}
             if n_f:
                 starts = np.cumsum([0] + ligand_num_atoms[:-1])
                 rows = torch.from_numpy((starts[:, None] + np.arange(n_f)[None, :]).reshape(-1)).to(device)
@@ -117,14 +137,14 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
                 init_ligand_pos[rows] = frag_pos.to(device).repeat(n_data, 1)
                 init_ligand_v = init_ligand_v.clone()
                 init_ligand_v[rows] = frag_v.to(device).repeat(n_data)
-                fixed['fixed_mask'] = mask
+                extra['fixed_mask'] = mask
                 if rng == 'cpu':
-                    fixed['fixed_noise_tape'] = (torch.randn(S + 1, n_lig, 3), torch.rand(S + 1, n_lig, model.num_classes))
+                    extra['fixed_noise_tape'] = (torch.randn(S + 1, n_lig, 3), torch.rand(S + 1, n_lig, model.num_classes))
 
             r = model.sample_diffusion(protein_pos=protein_pos, protein_v=protein_v, batch_protein=batch_protein,
                                        init_ligand_pos=init_ligand_pos, init_ligand_v=init_ligand_v, batch_ligand=batch_ligand,
                                        num_steps=num_steps, pos_only=pos_only, center_pos_mode=center_pos_mode, stack_traj=True,
-                                       noise_tape=tape, **fixed)
+                                       noise_tape=tape, **extra)
             cum = np.cumsum([0] + ligand_num_atoms)
             pos = r['pos'].cpu().numpy().astype(np.float64)
             all_pred_pos += [pos[cum[k]:cum[k + 1]] for k in range(n_data)]

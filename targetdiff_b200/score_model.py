@@ -169,6 +169,22 @@ def sublayer_code(cfg):
     return 1 << 24 | sync << 16 | nh << 8 | nx
 
 
+def check_time_seq(time_seq, T):
+    """`time_seq` as a list of ints, or ValueError unless it is tau_0 > tau_1 > ... > tau_{S-1} >= 0 with tau_0 = T - 1, 1 <= S <= T."""
+    seq = [int(x) for x in (time_seq.tolist() if hasattr(time_seq, 'tolist') else time_seq)]
+    if not seq:
+        raise ValueError('time_seq is empty')
+    if len(seq) > T:
+        raise ValueError('time_seq has %d steps, more than T = %d' % (len(seq), T))
+    if seq[0] != T - 1:
+        raise ValueError('time_seq must start at T - 1 = %d, not %d' % (T - 1, seq[0]))
+    if any(b >= a for a, b in zip(seq, seq[1:])):
+        raise ValueError('time_seq must be strictly decreasing')
+    if seq[-1] < 0:
+        raise ValueError('time_seq has a negative time %d' % seq[-1])
+    return seq
+
+
 def _counts_from_batch(batch, name):
     """Per-graph atom counts from a sorted PyG-style batch vector (host list)."""
     if batch.numel() == 0:
@@ -358,7 +374,7 @@ class ScorePosNet3D(nn.Module):
     @torch.no_grad()
     def sample_diffusion(self, protein_pos, protein_v, batch_protein, init_ligand_pos, init_ligand_v, batch_ligand,
                          num_steps=None, center_pos_mode=None, pos_only=False, noise_tape=None, seed=None, return_traj=True,
-                         stack_traj=False, fixed_mask=None, fixed_noise_tape=None):
+                         stack_traj=False, fixed_mask=None, fixed_noise_tape=None, time_seq=None):
         """The reverse-diffusion chain (reference models/molopt_score_model.py:633-703), executed entirely by libtdiff.so.
 
         Extensions over the reference signature (all optional): `noise_tape=(pos_noise [S,Nl,3], v_uniform [S,Nl,K])`
@@ -370,7 +386,17 @@ class ScorePosNet3D(nn.Module):
         Fixed atoms (fragment-conditioned sampling, DESIGN.md section 1): `fixed_mask` [Nl] bool holds the masked ligand atoms to the
         forward process of their `init_ligand_pos` / `init_ligand_v` rows (lab frame) through the chain; they end exactly there.
         `fixed_noise_tape=(pos_noise [S+1,Nl,3], v_uniform [S+1,Nl,K])` replaces their draws; it is required with `noise_tape` and
-        not allowed without it.  pos_traj / v_traj show the fixed rows as held, v0_traj / vt_traj what the network made of them."""
+        not allowed without it.  pos_traj / v_traj show the fixed rows as held, v0_traj / vt_traj what the network made of them.
+
+        Respaced sampling (DESIGN.md section 1): `time_seq` = tau_0 > ... > tau_{S-1} >= 0 with tau_0 = T - 1 runs S steps; step s
+        evaluates the network at tau_s and moves the state to tau_{s+1} (to tau_{S-1} - 1 at the last step) with the exact jump
+        posteriors.  `num_steps`, if given, must be S; tapes are [S, ...] (fixed tape [S+1, ...]) and trajectories [S, ...].
+        `sampling.respaced_time_seq(T, n)` makes an evenly spaced one.  Sample quality at fewer steps is not measured."""
+        if time_seq is not None:
+            time_seq = check_time_seq(time_seq, self.num_timesteps)
+            if num_steps is not None and int(num_steps) != len(time_seq):
+                raise ValueError('num_steps=%d disagrees with a time_seq of %d steps' % (int(num_steps), len(time_seq)))
+            num_steps = len(time_seq)
         if num_steps is None:
             num_steps = self.num_timesteps
         mode = {None: 0, 'none': 0, 'protein': 1}.get(center_pos_mode, None)
@@ -417,8 +443,12 @@ class ScorePosNet3D(nn.Module):
             if not pos_only:
                 v0_traj = torch.empty(S, Nl, K, device=dev)
                 vt_traj = torch.empty(S, Nl, K, device=dev)
-        _lib.check(lib.tdiff_sample(eng, S, _ptr(pos_noise), _ptr(v_uniform), ctypes.c_uint64(seed), _ptr(pos_traj), _ptr(v_traj),
-                                    _ptr(v0_traj), _ptr(vt_traj), int(bool(pos_only)), st))
+        if time_seq is None:
+            _lib.check(lib.tdiff_sample(eng, S, _ptr(pos_noise), _ptr(v_uniform), ctypes.c_uint64(seed), _ptr(pos_traj), _ptr(v_traj),
+                                        _ptr(v0_traj), _ptr(vt_traj), int(bool(pos_only)), st))
+        else:
+            _lib.check(lib.tdiff_sample_seq(eng, _lib.i32_array(time_seq), S, _ptr(pos_noise), _ptr(v_uniform), ctypes.c_uint64(seed),
+                                            _ptr(pos_traj), _ptr(v_traj), _ptr(v0_traj), _ptr(vt_traj), int(bool(pos_only)), st))
         out_pos = torch.empty(Nl, 3, device=dev)
         out_v = torch.empty(Nl, dtype=torch.int64, device=dev)
         _lib.check(lib.tdiff_get_ligand(eng, _ptr(out_pos), _ptr(out_v), 1, st))
