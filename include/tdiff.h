@@ -188,6 +188,24 @@ TDIFF_API int tdiff_sample_seq(tdiff_engine* e, const int32_t* h_time_seq, int n
                                uint64_t seed, float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only,
                                void* stream);
 
+/* Start-ligand sampling (an extension beyond the reference, DESIGN.md section 1): arms the next chains to start from the ligand state
+ * set by tdiff_set_ligand (the start ligand x0, v0, centred like any ligand) noised to the start time t_start in 0..T-1, and to run
+ * the reverse chain from there; t_start = -1 clears it.  While a start is armed:
+ *   the chain runs through tdiff_sample_seq only, and its time sequence must begin at tau_0 = t_start (the unit sequence
+ *   t_start, ..., 0 has t_start + 1 steps; a respaced one is allowed); tdiff_sample -> TDIFF_EINVAL.  Without a start
+ *   tdiff_sample_seq keeps requiring tau_0 = T - 1.
+ *   Before the first step, one launch (in place of the fixed set's) replaces every row: fixed rows (tdiff_set_fixed) by the sample
+ *   the fixed set gives them at t_start (draw 0 of the fixed-atom stream or tape); the others by a sample of q(x_{t_start} | x0),
+ *   q(v_{t_start} | v0) -- sqrt(alphas_cumprod[t_start]) x0 + sqrt(1 - alphas_cumprod[t_start]) eps with each product and the sum
+ *   rounded once, and Gumbel-max over q_v_pred(log_onehot(v0), t_start) -- the fixed set's formulas.  With pos_only the types stay
+ *   as set.  The steps are tdiff_sample_seq's, with the same launches.
+ * Noise: without tapes, the start draw of atom a comes from the sampler's Philox key on its own counters (a, 0, 0, 0x73747073 "stps")
+ * for positions and (a, 0, 1 + c/4, 0x73747476 "sttv") for class c; the sampler's and the fixed set's streams are unchanged.
+ * d_pos_noise [Nl,3] and d_v_uniform [Nl,K] (NULL under pos_only) give the start draw as a tape instead (borrowed pointers).  A chain
+ * takes either all of its tapes (step, fixed, start) or none (TDIFF_EINVAL otherwise).  Before tdiff_bind_batch -> TDIFF_ESTATE;
+ * t_start outside -1..T-1 -> TDIFF_EINVAL; tdiff_bind_batch clears the start. */
+TDIFF_API int tdiff_set_start(tdiff_engine* e, int t_start, const float* d_pos_noise, const float* d_v_uniform);
+
 /* Same loop through HOST buffers (the end-to-end path: H2D of the inputs, the chain, D2H of the results, all on
  * `stream`, synchronised before returning).  Equivalent of the device-facing part of sample_diffusion_ligand
  * (scripts/sample_diffusion.py:42-112) for one batch.  h_out_* may be NULL. */

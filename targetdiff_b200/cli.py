@@ -1,11 +1,14 @@
 """Command line for the sampling path (same arguments / outputs as the reference's scripts).
 
     python -m targetdiff_b200.cli sample_for_pocket configs/sampling.yml --pdb_path pocket.pdb [--num_samples N] [--result_path DIR]
-            [--fragment FILE]
+            [--fragment FILE | --start_ligand FILE]
         (reference scripts/sample_for_pocket.py:34-93: sample ligands into one pocket given as a PDB file; --fragment FILE, a .pt or
         .npz holding 'pos' [n,3] (the PDB's frame) and 'v' [n] class indices, grows every sample from that fragment: its atoms are
         the first n of each ligand and end exactly at 'pos' / 'v', see targetdiff_b200.sampling.  sample.pt then also holds
-        'fixed_ligand_atoms': n)
+        'fixed_ligand_atoms': n.  --start_ligand FILE, the same kind of file with an optional integer 'keep' [k] of atom indices,
+        starts every sample from that ligand noised to `sample.start_time` (required in the config with it) and keeps the 'keep'
+        atoms; sample.pt then also holds 'start_ligand' (pos, v), 'start_time', 'kept_atoms' and, with sample.respaced_steps,
+        'time_seq')
 
     [torchrun --nproc-per-node N -m] python -m targetdiff_b200.cli sample_pockets configs/sampling.yml --pocket_dir DIR | --pocket_list FILE
             [-i ID] [--schedule round_robin|longest_first] [--result_path DIR] [--num_samples N] [--batch_size B]
@@ -24,7 +27,7 @@ import sys
 
 import torch
 
-from .config import load_config, sampling_time_seq
+from .config import load_config, sampling_start, sampling_time_seq
 from .pocket import pdb_to_pocket_data
 from .sampling import sample_diffusion_ligand, seed_all
 from .score_model import ScorePosNet3D
@@ -120,6 +123,7 @@ def sample_pockets(argv):
     ap.add_argument('--num_samples', type=int)
     a = ap.parse_args(argv)
     config = load_config(a.config)
+    sampling_start(config.sample, None, False)      # start ligands are sample_for_pocket's only: refuses sample.start_time
     rank, world, local_rank = tdist.init_from_env()
     device = a.device or 'cuda:%d' % local_rank
     paths = list_pockets(a.pocket_dir, a.pocket_list)
@@ -147,8 +151,8 @@ def sample_pockets(argv):
     return done
 
 
-def load_fragment(path):
-    """(pos float32 [n,3], v int64 [n]) from a .pt (a dict) or .npz file with entries 'pos' and 'v'."""
+def _load_ligand_file(path, option):
+    """(entries dict, pos float32 [n,3], v int64 [n]) from a .pt (a dict) or .npz file with entries 'pos' and 'v'."""
     if path.endswith('.npz'):
         import numpy as np
         with np.load(path) as z:
@@ -156,15 +160,35 @@ def load_fragment(path):
     elif path.endswith('.pt'):
         d = torch.load(path, map_location='cpu', weights_only=True)
     else:
-        raise ValueError('--fragment %s: expected a .pt or .npz file' % path)
+        raise ValueError('%s %s: expected a .pt or .npz file' % (option, path))
     if not isinstance(d, dict) or 'pos' not in d or 'v' not in d:
-        raise ValueError("--fragment %s must hold 'pos' [n,3] and 'v' [n]" % path)
+        raise ValueError("%s %s must hold 'pos' [n,3] and 'v' [n]" % (option, path))
     pos = torch.as_tensor(d['pos']).float()
     v = torch.as_tensor(d['v'])
     if v.is_floating_point() or pos.dim() != 2 or pos.shape[1] != 3 or v.dim() != 1 or v.shape[0] != pos.shape[0] or v.shape[0] < 1:
-        raise ValueError("--fragment %s: 'pos' must be [n,3] and 'v' [n] integer class indices (n >= 1), got %s and %s %s"
-                         % (path, tuple(pos.shape), tuple(v.shape), v.dtype))
-    return pos, v.long()
+        raise ValueError("%s %s: 'pos' must be [n,3] and 'v' [n] integer class indices (n >= 1), got %s and %s %s"
+                         % (option, path, tuple(pos.shape), tuple(v.shape), v.dtype))
+    return d, pos, v.long()
+
+
+def load_fragment(path):
+    """(pos float32 [n,3], v int64 [n]) from a .pt (a dict) or .npz file with entries 'pos' and 'v'."""
+    _, pos, v = _load_ligand_file(path, '--fragment')
+    return pos, v
+
+
+def load_start_ligand(path):
+    """(pos float32 [n,3], v int64 [n], keep int64 [k] or None) from a .pt (a dict) or .npz file with entries 'pos', 'v' and an
+    optional 'keep' of atom indices to keep (sample_diffusion_ligand checks their range and uniqueness)."""
+    d, pos, v = _load_ligand_file(path, '--start_ligand')
+    keep = d.get('keep')
+    if keep is not None:
+        keep = torch.as_tensor(keep)
+        if keep.is_floating_point() or keep.is_complex() or keep.dtype == torch.bool or keep.dim() != 1:
+            raise ValueError("--start_ligand %s: 'keep' must be a 1-D array of integer atom indices, got %s %s"
+                             % (path, tuple(keep.shape), keep.dtype))
+        keep = keep.long()
+    return pos, v, keep
 
 
 def sample_for_pocket(argv):
@@ -176,24 +200,37 @@ def sample_for_pocket(argv):
     ap.add_argument('--result_path', type=str, default='./outputs_pdb')
     ap.add_argument('--num_samples', type=int)
     ap.add_argument('--fragment', type=str, help=".pt / .npz with 'pos' [n,3] and 'v' [n]: every sample grows from this fragment")
+    ap.add_argument('--start_ligand', type=str, help=".pt / .npz with 'pos' [n,3], 'v' [n] and optional 'keep' [k]: every sample starts "
+                                                     "from this ligand noised to sample.start_time")
     a = ap.parse_args(argv)
+    if a.fragment and a.start_ligand:
+        raise ValueError('--fragment cannot be combined with --start_ligand: keep atoms of the start ligand with its \'keep\' entry')
     config = load_config(a.config)
     fragment = load_fragment(a.fragment) if a.fragment else None
+    start = load_start_ligand(a.start_ligand) if a.start_ligand else None
     seed_all(config.sample.seed)
     model = _load_model(config, a.device)
-    time_seq = _time_seq(config, model)
+    start_time, start_seq = sampling_start(config.sample, model.num_timesteps, start is not None)
+    time_seq = _time_seq(config, model) if start is None else start_seq
     data = pdb_to_pocket_data(a.pdb_path)
     n = a.num_samples if a.num_samples is not None else config.sample.num_samples
+    kw = {} if start is None else dict(start_ligand=start[:2], start_time=start_time, keep_atoms=start[2])
     outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=a.device,
                                       num_steps=config.sample.num_steps if time_seq is None else None, pos_only=config.sample.pos_only,
                                       center_pos_mode=config.sample.center_pos_mode, sample_num_atoms=config.sample.sample_num_atoms,
-                                      fixed_ligand=fragment, time_seq=time_seq)
+                                      fixed_ligand=fragment, time_seq=time_seq, **kw)
     os.makedirs(a.result_path, exist_ok=True)
     shutil.copyfile(a.config, os.path.join(a.result_path, 'sample.yml'))
     result = build_result(data, outputs)
     if fragment is not None:
         result['fixed_ligand_atoms'] = int(fragment[1].shape[0])
-    if time_seq is not None:
+    if start is not None:
+        result['start_ligand'] = (start[0], start[1])
+        result['start_time'] = start_time
+        result['kept_atoms'] = [] if start[2] is None else start[2].tolist()
+        if config.sample.get('respaced_steps') is not None:
+            result['time_seq'] = time_seq
+    elif time_seq is not None:
         result['time_seq'] = time_seq
     torch.save(result, os.path.join(a.result_path, 'sample.pt'))
     print('Sample done! %d molecules, %.1f s' % (len(outputs[0]), sum(outputs[-1])))

@@ -61,6 +61,32 @@ def sampling_time_seq(sample, T):
     return respaced_time_seq(T, n)
 
 
+def sampling_start(sample, T, start_ligand):
+    """(start time t0, time sequence) of a chain from a start ligand (an extension beyond the reference's sampling.yml), or
+    (None, None) without one (`start_ligand` False).  `sample.start_time` is required with a start ligand and refused without one;
+    the sequence is t0, t0 - 1, ..., 0, or with `sample.respaced_steps` = n sampling.respaced_time_seq(T, n, start=t0).  ValueError
+    with a `sample.num_steps` other than T, as for sampling_time_seq: the start time sets the chain's length."""
+    t0 = sample.get('start_time')
+    if not start_ligand:
+        if t0 is not None:
+            raise ValueError('sample.start_time=%s needs a start ligand (--start_ligand)' % (t0,))
+        return None, None
+    if t0 is None:
+        raise ValueError('a start ligand (--start_ligand) needs sample.start_time in the config')
+    t0 = int(t0)
+    if not 0 <= t0 <= T - 1:
+        raise ValueError('sample.start_time=%d outside 0..T-1 = %d' % (t0, T - 1))
+    steps = sample.get('num_steps', T)
+    if steps is not None and int(steps) != T:
+        raise ValueError('sample.start_time=%d cannot be combined with sample.num_steps=%s (the start time sets the chain; '
+                         'leave num_steps at T = %d)' % (t0, steps, T))
+    n = sample.get('respaced_steps')
+    if n is None:
+        return t0, list(range(t0, -1, -1))
+    from .sampling import respaced_time_seq
+    return t0, respaced_time_seq(T, n, start=t0)
+
+
 # Values the sm_90a engine implements; anything else is rejected loudly (SURVEY.md 8(b) "should-reject-clearly").
 _SUPPORTED = dict(model_mean_type=('C0', 'noise'), beta_schedule=('sigmoid', 'linear', 'quad', 'const', 'jsd', 'cosine'),
                   v_beta_schedule=('cosine',), node_indicator=(True,), model_type=('uni_o2',),

@@ -124,6 +124,9 @@ struct tdiff_engine {
   bool has_fixed = false;
   DevBuf fix_mask, fix_pos, fix_v;
   const float *fix_pos_noise = nullptr, *fix_v_uniform = nullptr;
+  // start chains (tdiff_set_start): start_t = -1 none; the borrowed start tape [Nl,3] / [Nl,K] or NULL; cleared by tdiff_bind_batch
+  int start_t = -1;
+  const float *start_pos_noise = nullptr, *start_v_uniform = nullptr;
   // respaced chains (tdiff_sample_seq): double prefix sums over i = 0..t of log(1 - betas[i]) (= log alphas_cumprod[t]) and of
   // log_alphas_v[i]; the per-step tables of the current chain: seq_t, seq_p [S] int | c0, ct, logvar, la, l1ma [S] fp32
   std::vector<double> cum_log_a, cum_log_av;
@@ -669,6 +672,7 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   node_ptr[B] = n; prot_ptr[B] = p;
   e->bound = false; e->has_ligand = false; e->have_graph = false; e->have_prev = false;
   e->has_fixed = false; e->fix_pos_noise = nullptr; e->fix_v_uniform = nullptr;
+  e->start_t = -1; e->start_pos_noise = nullptr; e->start_v_uniform = nullptr;
   e->B = B; e->N = (int)N; e->Np = (int)Np; e->Nl = (int)Nl; e->max_ng = max_ng;
   const size_t slots = (size_t)N * K;
   int bad = 0;
@@ -812,6 +816,17 @@ extern "C" int tdiff_set_fixed_tape(tdiff_engine* e, const float* d_pos_noise, c
   if (!e || !e->bound) return set_err(TDIFF_ESTATE, "set_fixed_tape before bind_batch");
   e->fix_pos_noise = d_pos_noise;
   e->fix_v_uniform = d_pos_noise ? d_v_uniform : nullptr;
+  return TDIFF_OK;
+}
+
+extern "C" int tdiff_set_start(tdiff_engine* e, int t_start, const float* d_pos_noise, const float* d_v_uniform) {
+  if (!e || !e->bound) return set_err(TDIFF_ESTATE, "set_start before bind_batch");
+  const int T = e->cfg.num_timesteps;
+  if (t_start < -1 || t_start > T - 1) return set_err(TDIFF_EINVAL, "set_start: t_start=%d outside -1..%d", t_start, T - 1);
+  const bool on = t_start >= 0;
+  e->start_t = t_start;
+  e->start_pos_noise = on ? d_pos_noise : nullptr;
+  e->start_v_uniform = on && d_pos_noise ? d_v_uniform : nullptr;
   return TDIFF_OK;
 }
 
@@ -1226,10 +1241,15 @@ int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const 
                  float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only, void* stream) {
   if (!e || !e->bound || !e->has_ligand) return set_err(TDIFF_ESTATE, "sample needs bind_batch + set_ligand first");
   const int T = e->cfg.num_timesteps;
+  const bool start = e->start_t >= 0;
+  if (start && !time_seq)
+    return set_err(TDIFF_EINVAL, "a start is armed (tdiff_set_start, t_start=%d): run the chain with tdiff_sample_seq from t_start", e->start_t);
   if (num_steps < 0 || num_steps > T) return set_err(TDIFF_EINVAL, "num_steps=%d outside 0..%d", num_steps, T);
   if (time_seq) {
     if (num_steps < 1) return set_err(TDIFF_EINVAL, "time sequence: empty (num_steps=%d)", num_steps);
-    if (time_seq[0] != T - 1) return set_err(TDIFF_EINVAL, "time sequence: starts at %d, not at T - 1 = %d", time_seq[0], T - 1);
+    if (start && time_seq[0] != e->start_t)
+      return set_err(TDIFF_EINVAL, "time sequence: starts at %d, not at the start time t_start = %d", time_seq[0], e->start_t);
+    if (!start && time_seq[0] != T - 1) return set_err(TDIFF_EINVAL, "time sequence: starts at %d, not at T - 1 = %d", time_seq[0], T - 1);
     for (int s = 1; s < num_steps; ++s) {
       if (time_seq[s] >= time_seq[s - 1])
         return set_err(TDIFF_EINVAL, "time sequence: not strictly decreasing at step %d (%d after %d)", s, time_seq[s], time_seq[s - 1]);
@@ -1245,12 +1265,19 @@ int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const 
     if (d_pos_noise && !pos_only && !e->fix_v_uniform)
       return set_err(TDIFF_EINVAL, "the fixed-atom tape needs v_uniform unless pos_only");
   }
+  if (start) {             // the same rule for the start tape
+    if ((d_pos_noise != nullptr) != (e->start_pos_noise != nullptr))
+      return set_err(TDIFF_EINVAL, d_pos_noise ? "a start with a noise tape needs a start tape (tdiff_set_start)"
+                                               : "a start tape is set but the chain has no noise tape (clear it, or pass both)");
+    if (d_pos_noise && !pos_only && !e->start_v_uniform)
+      return set_err(TDIFF_EINVAL, "the start tape needs v_uniform unless pos_only");
+  }
   cudaStream_t st = (cudaStream_t)stream;
   CK(cudaSetDevice(e->device));
   if (num_steps == 0) return TDIFF_OK;
   TdStepArgs A;
   memset(&A, 0, sizeof(A));
-  A.n_lig = e->Nl; A.n_classes = e->cfg.num_classes; A.t_start = T - 1; A.pos_only = pos_only;
+  A.n_lig = e->Nl; A.n_classes = e->cfg.num_classes; A.t_start = start ? e->start_t : T - 1; A.pos_only = pos_only;
   A.step = e->step.as<int>(); A.lig_node = e->lig_node.as<int>(); A.lig_graph = e->lig_graph.as<int>();
   A.logits = e->logits.as<float>(); A.offset = e->offset.as<float4>();
   A.c0 = e->t_c0; A.ct = e->t_ct; A.logvar = e->t_logvar; A.la_v = e->t_la; A.l1ma_v = e->t_l1ma; A.lca_v = e->t_lca; A.l1mca_v = e->t_l1mca;
@@ -1263,6 +1290,7 @@ int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const 
     A.fix_mask = e->fix_mask.as<unsigned char>(); A.fix_pos = e->fix_pos.as<float4>(); A.fix_v = e->fix_v.as<int>(); A.ac = e->t_ac;
     A.fix_pos_noise = e->fix_pos_noise; A.fix_v_uniform = e->fix_v_uniform;
   }
+  if (start) { A.ac = e->t_ac; A.start_pos_noise = e->start_pos_noise; A.start_v_uniform = e->start_v_uniform; }
   if (time_seq) {
     std::vector<int> it;
     std::vector<float> ft;
@@ -1277,7 +1305,10 @@ int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const 
     A.seq_c0 = sf; A.seq_ct = sf + S; A.seq_logvar = sf + 2 * S; A.seq_la = sf + 3 * S; A.seq_l1ma = sf + 4 * S;
   }
   CK(cudaMemsetAsync(e->step.p, 0, sizeof(int), st));
-  if (e->has_fixed) {      // the chain's one extra launch: fixed rows <- q(x_{T-1} | x0_f), q(v_{T-1} | v0_f)
+  if (start) {             // the chain's one extra launch: every row <- a sample of the forward process at t_start (DESIGN.md section 1)
+    td_launch_start_init(A, st);
+    e->launches += 1;
+  } else if (e->has_fixed) {      // the chain's one extra launch: fixed rows <- q(x_{T-1} | x0_f), q(v_{T-1} | v0_f)
     td_launch_fixed_init(A, st);
     e->launches += 1;
   }

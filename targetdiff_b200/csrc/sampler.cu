@@ -31,26 +31,46 @@ __device__ __forceinline__ float log_add_exp_f(float a, float b) {
 // Philox domain words of the fixed-atom stream ("fxps", "fxtv"), distinct from the sampler's "pst\0" / "vuni" (oracle/fixed_atoms.py)
 #define TD_FIX_POS_DOMAIN 0x66787073u
 #define TD_FIX_TYPE_DOMAIN 0x66787476u
+// Philox domain words of the start-ligand stream ("stps", "sttv"), distinct from the four above (oracle/start_ligand.py)
+#define TD_START_POS_DOMAIN 0x73747073u
+#define TD_START_TYPE_DOMAIN 0x73747476u
 
-// Fixed atom `a` (DESIGN.md section 1, fixed atoms): a sample of q(x_tm | x0_f) and q(v_tm | v0_f) from draw `d` of the fixed-atom
-// stream (d = 0 before the first step, d = j + 1 after step j), or x0_f / v0_f exactly when tm < 0.  Position
+// Sources of forward_sample: x0 / v0, the tapes and the Philox domain words of the fixed-atom stream and of the start stream
+struct TdFixedSource {
+  static constexpr unsigned kPosDomain = TD_FIX_POS_DOMAIN, kTypeDomain = TD_FIX_TYPE_DOMAIN;
+  static __device__ __forceinline__ const float4* x0(const TdStepArgs& A) { return A.fix_pos; }
+  static __device__ __forceinline__ const int* v0(const TdStepArgs& A) { return A.fix_v; }
+  static __device__ __forceinline__ const float* pos_tape(const TdStepArgs& A) { return A.fix_pos_noise; }
+  static __device__ __forceinline__ const float* v_tape(const TdStepArgs& A) { return A.fix_v_uniform; }
+};
+struct TdStartSource {            // the start ligand is the chain's own state before the start draw
+  static constexpr unsigned kPosDomain = TD_START_POS_DOMAIN, kTypeDomain = TD_START_TYPE_DOMAIN;
+  static __device__ __forceinline__ const float4* x0(const TdStepArgs& A) { return A.lig_pos; }
+  static __device__ __forceinline__ const int* v0(const TdStepArgs& A) { return A.lig_v; }
+  static __device__ __forceinline__ const float* pos_tape(const TdStepArgs& A) { return A.start_pos_noise; }
+  static __device__ __forceinline__ const float* v_tape(const TdStepArgs& A) { return A.start_v_uniform; }
+};
+
+// Row `a`: a sample of q(x_tm | x0) and q(v_tm | v0) with x0 / v0 from `Src`, from draw `d` of its stream (the sampler's key and counter
+// layout on Src's domain words) or rows d of its tapes [., Nl, 3] / [., Nl, K]; x0 / v0 exactly when tm < 0.  Position
 // sqrt(ac) x0 + sqrt(1 - ac) eps with every product and the sum rounded once, as the reference's perturbation
 // (models/molopt_score_model.py:500-504); type: Gumbel-max over the unnormalised q_v_pred(log_onehot(v0), tm) (q_v_sample, :394-398).
 // With pos_only the type is left as it is.
-__device__ __forceinline__ void fixed_sample(const TdStepArgs& A, int a, int d, int tm, float4& x, int& v) {
-  const float4 x0 = A.fix_pos[a];
+template <class Src>
+__device__ __forceinline__ void forward_sample(const TdStepArgs& A, int a, int d, int tm, float4& x, int& v) {
+  const float4 x0 = Src::x0(A)[a];
   if (tm < 0) {
     x = make_float4(x0.x, x0.y, x0.z, 1.0f);
-    if (!A.pos_only) v = A.fix_v[a];
+    if (!A.pos_only) v = Src::v0(A)[a];
     return;
   }
   const uint2 key = make_uint2((unsigned)A.seed, (unsigned)(A.seed >> 32));
   float nz[3];
-  if (A.fix_pos_noise) {
-    const float* pn = A.fix_pos_noise + ((size_t)d * A.n_lig + a) * 3;
+  if (Src::pos_tape(A)) {
+    const float* pn = Src::pos_tape(A) + ((size_t)d * A.n_lig + a) * 3;
     nz[0] = pn[0]; nz[1] = pn[1]; nz[2] = pn[2];
   } else {
-    const uint4 r0 = philox4x32_10(make_uint4((unsigned)a, (unsigned)d, 0u, TD_FIX_POS_DOMAIN), key);
+    const uint4 r0 = philox4x32_10(make_uint4((unsigned)a, (unsigned)d, 0u, Src::kPosDomain), key);
     const float u0 = 1.0f - u01(r0.x), u1 = u01(r0.y), u2 = 1.0f - u01(r0.z), u3 = u01(r0.w);
     const float ra = sqrtf(-2.0f * logf(u0)), rb = sqrtf(-2.0f * logf(u2));
     nz[0] = ra * cospif(2.0f * u1); nz[1] = ra * sinpif(2.0f * u1); nz[2] = rb * cospif(2.0f * u3);
@@ -62,18 +82,18 @@ __device__ __forceinline__ void fixed_sample(const TdStepArgs& A, int a, int d, 
   x.z = __fadd_rn(__fmul_rn(sa, x0.z), __fmul_rn(sb, nz[2]));
   x.w = 1.0f;
   if (A.pos_only) return;
-  const int K = A.n_classes, v0 = A.fix_v[a];
+  const int K = A.n_classes, v0 = Src::v0(A)[a];
   const float lca = A.lca_v[tm], l1mca = A.l1mca_v[tm] - A.log_k;
   const float log_eps = -69.07755279f;                                     // logf(1e-30f): index_to_log_onehot's clamp
   float best = -INFINITY;
   int vbest = 0;
   for (int c0 = 0; c0 < K; c0 += 4) {
     float u[4];
-    if (A.fix_v_uniform) {
-      const float* vu = A.fix_v_uniform + ((size_t)d * A.n_lig + a) * K;
+    if (Src::v_tape(A)) {
+      const float* vu = Src::v_tape(A) + ((size_t)d * A.n_lig + a) * K;
       for (int j = 0; j < 4 && c0 + j < K; ++j) u[j] = vu[c0 + j];
     } else {
-      const uint4 r = philox4x32_10(make_uint4((unsigned)a, (unsigned)d, 1u + (unsigned)(c0 >> 2), TD_FIX_TYPE_DOMAIN), key);
+      const uint4 r = philox4x32_10(make_uint4((unsigned)a, (unsigned)d, 1u + (unsigned)(c0 >> 2), Src::kTypeDomain), key);
       u[0] = u01(r.x); u[1] = u01(r.y); u[2] = u01(r.z); u[3] = u01(r.w);
     }
     for (int j = 0; j < 4 && c0 + j < K; ++j) {
@@ -84,6 +104,12 @@ __device__ __forceinline__ void fixed_sample(const TdStepArgs& A, int a, int d, 
     }
   }
   v = vbest;
+}
+
+// Fixed atom `a` (DESIGN.md section 1, fixed atoms): a sample of q(x_tm | x0_f) and q(v_tm | v0_f) from draw `d` of the fixed-atom
+// stream or tape (d = 0 before the first step, d = j + 1 after step j), or x0_f / v0_f exactly when tm < 0.
+__device__ __forceinline__ void fixed_sample(const TdStepArgs& A, int a, int d, int tm, float4& x, int& v) {
+  forward_sample<TdFixedSource>(A, a, d, tm, x, v);
 }
 
 // kFixed = false (no fixed set) compiles to the step as it was before fixed atoms existed.  kSeq = true runs step s of a respaced
@@ -228,6 +254,23 @@ __global__ void fixed_init_kernel(TdStepArgs A) {
 }
 void td_launch_fixed_init(const TdStepArgs& A, cudaStream_t st) {
   if (A.n_lig > 0) fixed_init_kernel<<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
+}
+
+// start chain (tdiff_set_start), once before its first step, in place of fixed_init_kernel: every row <- a sample at t_start.  Fixed
+// rows as fixed_init_kernel gives them (draw 0 of the fixed-atom stream); the others from the start stream with their own state, the
+// start ligand, as x0 / v0 -- counters (a, 0, 0, "stps") and (a, 0, 1 + c/4, "sttv"), or the start tape pos [Nl,3], v [Nl,K].
+__global__ void start_init_kernel(TdStepArgs A) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= A.n_lig) return;
+  float4 x;
+  int v = A.lig_v[a];
+  if (A.fix_mask && A.fix_mask[a]) fixed_sample(A, a, 0, A.t_start, x, v);
+  else forward_sample<TdStartSource>(A, a, 0, A.t_start, x, v);
+  A.lig_pos[a] = x;
+  A.lig_v[a] = v;
+}
+void td_launch_start_init(const TdStepArgs& A, cudaStream_t st) {
+  if (A.n_lig > 0) start_init_kernel<<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
 }
 
 // fixed set in (tdiff_set_fixed): positions and classes are read at masked rows only; lab frame -> centred like set_ligand_kernel

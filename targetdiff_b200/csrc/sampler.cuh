@@ -37,10 +37,14 @@ struct TdStepArgs {
   const int* seq_p;                // [S] the time step s moves to: tau_{s+1}, or tau_{S-1} - 1 at the last step
   const float *seq_c0, *seq_ct, *seq_logvar;   // [S] position posterior of the jump t -> p (the checkpoint's tables at t on unit steps)
   const float *seq_la, *seq_l1ma;  // [S] lambda = log of the type schedule's transition probability p -> t, log(1 - e^lambda + 1e-40)
+  // start chain (tdiff_set_start): the start draw's tape, read by start_init_kernel only
+  const float* start_pos_noise;    // [Nl,3] or NULL (Philox, START_POS domain)
+  const float* start_v_uniform;    // [Nl,K] or NULL (Philox, START_TYPE domain)
 };
 
 void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st);
 void td_launch_fixed_init(const TdStepArgs& A, cudaStream_t st);
+void td_launch_start_init(const TdStepArgs& A, cudaStream_t st);
 void td_launch_set_fixed(const unsigned char* mask, const float* pos, const long long* v, const int* lig_graph, const float4* offset,
                          int apply_center, int n, int n_classes, unsigned char* fix_mask, float4* fix_pos, int* fix_v, int* err,
                          cudaStream_t st);

@@ -22,7 +22,16 @@ keeps the reference ligand's types and cannot take a fragment.
 Respaced sampling (an extension beyond the reference, DESIGN.md section 1).  `time_seq` (e.g. `respaced_time_seq(T, 100)`) runs the
 chain on that decreasing subsequence of timesteps with the exact jump posteriors (ScorePosNet3D.sample_diffusion(time_seq=...)).
 Under rng='cpu' the tape has S = len(time_seq) steps in the reference's interleaved order, then comes the fixed tape [S+1, ...].
-Whether a checkpoint's molecules keep their quality at fewer steps has not been measured."""
+Whether a checkpoint's molecules keep their quality at fewer steps has not been measured.
+
+Start-ligand sampling (an extension beyond the reference, DESIGN.md section 1).  `start_ligand=(pos [n,3] lab frame, v [n] class
+indices)` with `start_time` = t0 starts every sample from that ligand noised to t0 and runs the reverse chain from t0
+(ScorePosNet3D.sample_diffusion(start_time=...)): by default t0, t0 - 1, ..., 0, or `time_seq` from t0 (e.g. respaced_time_seq(T, n,
+start=t0)).  Every sample has the start ligand's n atoms (`sample_num_atoms` is not read), and no initial N(0,1) or uniform draws are
+made.  `keep_atoms` (indices into the start ligand) become fixed rows, held to the forward process of their start positions and types.
+Under rng='cpu' each batch draws, in this order, the start tape randn(Nl, 3), rand(Nl, K) (the uniforms skipped under pos_only), the
+step tape in the reference's interleaved order, and with kept atoms the fixed tape randn(S+1, Nl, 3), rand(S+1, Nl, K) (the uniforms
+skipped under pos_only).  With pos_only the types are the start ligand's.  Sample quality from a start ligand has not been measured."""
 import time
 
 import numpy as np
@@ -40,15 +49,64 @@ def seed_all(seed):
     random.seed(seed)
 
 
-def respaced_time_seq(T, n):
+def respaced_time_seq(T, n, start=None):
     """n timesteps spaced evenly from T - 1 down to 0, each rounded to the nearest integer (half to even): a strictly decreasing
-    time sequence for ScorePosNet3D.sample_diffusion(time_seq=...).  n = T gives the default chain T-1, ..., 0."""
+    time sequence for ScorePosNet3D.sample_diffusion(time_seq=...).  n = T gives the default chain T-1, ..., 0.  With a start time
+    `start` in 0..T-1 the sequence runs from `start` down to 0 instead, with 2 <= n <= start + 1 (n = 1 when start = 0)."""
     T, n = int(T), int(n)
-    if not 2 <= n <= T:
-        raise ValueError('respaced steps must lie in 2..T = %d, got %d' % (T, n))
-    seq = [int(x) for x in np.rint(np.linspace(T - 1, 0, n))]
-    assert seq[0] == T - 1 and seq[-1] == 0 and all(b < a for a, b in zip(seq, seq[1:]))
+    if start is None:
+        if not 2 <= n <= T:
+            raise ValueError('respaced steps must lie in 2..T = %d, got %d' % (T, n))
+        top = T - 1
+    else:
+        top = int(start)
+        if not 0 <= top <= T - 1:
+            raise ValueError('start time %d outside 0..T-1 = %d' % (top, T - 1))
+        lo = 1 if top == 0 else 2
+        if not lo <= n <= top + 1:
+            raise ValueError('respaced steps from start time %d must lie in %d..%d, got %d' % (top, lo, top + 1, n))
+    seq = [int(x) for x in np.rint(np.linspace(top, 0, n))]
+    assert seq[0] == top and seq[-1] == 0 and all(b < a for a, b in zip(seq, seq[1:]))
     return seq
+
+
+def _check_start(model, start_ligand, start_time, keep_atoms, fixed_ligand):
+    """(pos [n,3] float32, v [n] int64, t0, keep [k] int64) of a start ligand, or None without one; ValueError for what
+    sample_diffusion_ligand refuses."""
+    if start_ligand is None:
+        if start_time is not None or keep_atoms is not None:
+            raise ValueError('start_time and keep_atoms need a start_ligand')
+        return None
+    if start_time is None:
+        raise ValueError('a start_ligand needs a start_time')
+    if fixed_ligand is not None:
+        raise ValueError('fixed_ligand cannot be combined with start_ligand: keep atoms of the start ligand with keep_atoms instead')
+    T = model.num_timesteps
+    t0 = int(start_time)
+    if not 0 <= t0 <= T - 1:
+        raise ValueError('start_time %d outside 0..T-1 = %d' % (t0, T - 1))
+    pos = torch.as_tensor(start_ligand[0]).detach().cpu().float()
+    v = torch.as_tensor(start_ligand[1]).detach().cpu()
+    n = v.shape[0] if v.dim() == 1 else -1
+    if v.is_floating_point() or pos.dim() != 2 or tuple(pos.shape) != (n, 3) or n < 1:
+        raise ValueError('start_ligand must be (pos [n,3], v [n] integer classes) with n >= 1; got shapes %s, %s'
+                         % (tuple(pos.shape), tuple(v.shape)))
+    v = v.long()
+    if int(v.min()) < 0 or int(v.max()) >= model.num_classes:
+        raise ValueError('start_ligand classes must lie in 0..%d' % (model.num_classes - 1))
+    keep = torch.zeros(0, dtype=torch.long)
+    if keep_atoms is not None:
+        keep = torch.as_tensor(keep_atoms).detach().cpu().reshape(-1)
+        if keep.is_floating_point():
+            raise ValueError('keep_atoms must be integer indices into the start ligand')
+        keep = keep.long()
+        if len(keep) and (int(keep.min()) < 0 or int(keep.max()) >= n):
+            raise ValueError('keep_atoms must lie in 0..%d' % (n - 1))
+        if len(torch.unique(keep)) != len(keep):
+            raise ValueError('keep_atoms must be unique')
+        if len(keep) >= n:
+            raise ValueError('keep_atoms must leave at least one of the %d start atoms free' % n)
+    return pos, v, t0, keep
 
 
 def _split(arr, cum, n_data):
@@ -56,11 +114,15 @@ def _split(arr, cum, n_data):
 
 
 def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cuda:0', num_steps=None, pos_only=False,
-                            center_pos_mode='protein', sample_num_atoms='prior', rng='device', fixed_ligand=None, time_seq=None):
+                            center_pos_mode='protein', sample_num_atoms='prior', rng='device', fixed_ligand=None, time_seq=None,
+                            start_ligand=None, start_time=None, keep_atoms=None):
     if rng not in ('device', 'cpu'):
         raise ValueError("rng must be 'device' or 'cpu'")
+    start = _check_start(model, start_ligand, start_time, keep_atoms, fixed_ligand)
+    if start is not None and time_seq is None:
+        time_seq = list(range(start[2], -1, -1))
     if time_seq is not None:
-        time_seq = check_time_seq(time_seq, model.num_timesteps)
+        time_seq = check_time_seq(time_seq, model.num_timesteps, start=None if start is None else start[2])
         if num_steps is not None and int(num_steps) != len(time_seq):
             raise ValueError('num_steps=%d disagrees with a time_seq of %d steps' % (int(num_steps), len(time_seq)))
     n_f = 0
@@ -91,7 +153,9 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
         t1 = time.time()
         with torch.no_grad():
             batch_protein = torch.repeat_interleave(torch.arange(n_data, device=device), n_prot)
-            if sample_num_atoms == 'prior':
+            if start is not None:                                       # every sample is the start ligand
+                ligand_num_atoms = [len(start[1])] * n_data
+            elif sample_num_atoms == 'prior':
                 pocket_size = atom_num.get_space_size(protein_pos_cpu.numpy())
                 ligand_num_atoms = [int(atom_num.sample_atom_num(pocket_size)) for _ in range(n_data)]
             elif sample_num_atoms == 'range':
@@ -109,15 +173,23 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
             # init ligand pos: pocket centre + N(0, 1)   (reference :61-63; scatter_mean = sequential sum / count, every clone
             # of the pocket has the same centre)
             n_lig = len(batch_ligand)
-            center = (torch.zeros(1, 3).index_add_(0, torch.zeros(n_prot, dtype=torch.long), protein_pos_cpu) / max(n_prot, 1)).to(device)
-            draw_dev = device if rng == 'device' else 'cpu'
-            init_ligand_pos = center.expand(n_lig, 3) + torch.randn(n_lig, 3, device=draw_dev).to(device)
-            # init ligand v (reference :66-70)
-            if pos_only:
-                init_ligand_v = data.ligand_atom_feature_full.to(device).repeat(n_data)
+            extra = {} if time_seq is None else {'time_seq': time_seq}
+            if start is not None:                                       # the clean start ligand; the engine noises it to t0
+                init_ligand_pos = start[0].to(device).repeat(n_data, 1)
+                init_ligand_v = start[1].to(device).repeat(n_data)
+                extra['start_time'] = start[2]
+                if rng == 'cpu':
+                    extra['start_noise_tape'] = (torch.randn(n_lig, 3), None if pos_only else torch.rand(n_lig, model.num_classes))
             else:
-                uniform_logits = torch.zeros(n_lig, model.num_classes, device=draw_dev)
-                init_ligand_v = log_sample_categorical(uniform_logits).to(device)
+                center = (torch.zeros(1, 3).index_add_(0, torch.zeros(n_prot, dtype=torch.long), protein_pos_cpu) / max(n_prot, 1)).to(device)
+                draw_dev = device if rng == 'device' else 'cpu'
+                init_ligand_pos = center.expand(n_lig, 3) + torch.randn(n_lig, 3, device=draw_dev).to(device)
+                # init ligand v (reference :66-70)
+                if pos_only:
+                    init_ligand_v = data.ligand_atom_feature_full.to(device).repeat(n_data)
+                else:
+                    uniform_logits = torch.zeros(n_lig, model.num_classes, device=draw_dev)
+                    init_ligand_v = log_sample_categorical(uniform_logits).to(device)
             tape = None
             if rng == 'cpu':
                 S = len(time_seq) if time_seq is not None else model.num_timesteps if num_steps is None else int(num_steps)
@@ -128,7 +200,15 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
                     if not pos_only:
                         vu[st] = torch.rand(n_lig, model.num_classes)
                 tape = (pn, vu)
-            extra = {} if time_seq is None else {'time_seq': time_seq}
+            if start is not None and len(start[3]):
+                starts = np.cumsum([0] + ligand_num_atoms[:-1])
+                rows = torch.from_numpy((starts[:, None] + start[3].numpy()[None, :]).reshape(-1)).to(device)
+                mask = torch.zeros(n_lig, dtype=torch.bool, device=device)
+                mask[rows] = True
+                extra['fixed_mask'] = mask
+                if rng == 'cpu':
+                    extra['fixed_noise_tape'] = (torch.randn(S + 1, n_lig, 3),
+                                                 None if pos_only else torch.rand(S + 1, n_lig, model.num_classes))
             if n_f:
                 starts = np.cumsum([0] + ligand_num_atoms[:-1])
                 rows = torch.from_numpy((starts[:, None] + np.arange(n_f)[None, :]).reshape(-1)).to(device)

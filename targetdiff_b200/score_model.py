@@ -169,15 +169,22 @@ def sublayer_code(cfg):
     return 1 << 24 | sync << 16 | nh << 8 | nx
 
 
-def check_time_seq(time_seq, T):
-    """`time_seq` as a list of ints, or ValueError unless it is tau_0 > tau_1 > ... > tau_{S-1} >= 0 with tau_0 = T - 1, 1 <= S <= T."""
+def check_time_seq(time_seq, T, start=None):
+    """`time_seq` as a list of ints, or ValueError unless it is tau_0 > tau_1 > ... > tau_{S-1} >= 0 with tau_0 = T - 1, 1 <= S <= T;
+    with a start time `start` (a chain from a start ligand, DESIGN.md section 1), tau_0 = start instead, in 0..T-1."""
     seq = [int(x) for x in (time_seq.tolist() if hasattr(time_seq, 'tolist') else time_seq)]
     if not seq:
         raise ValueError('time_seq is empty')
     if len(seq) > T:
         raise ValueError('time_seq has %d steps, more than T = %d' % (len(seq), T))
-    if seq[0] != T - 1:
-        raise ValueError('time_seq must start at T - 1 = %d, not %d' % (T - 1, seq[0]))
+    if start is None:
+        if seq[0] != T - 1:
+            raise ValueError('time_seq must start at T - 1 = %d, not %d' % (T - 1, seq[0]))
+    else:
+        if not 0 <= int(start) <= T - 1:
+            raise ValueError('start time %d outside 0..T-1 = %d' % (int(start), T - 1))
+        if seq[0] != int(start):
+            raise ValueError('time_seq must start at the start time %d, not %d' % (int(start), seq[0]))
     if any(b >= a for a, b in zip(seq, seq[1:])):
         raise ValueError('time_seq must be strictly decreasing')
     if seq[-1] < 0:
@@ -374,7 +381,7 @@ class ScorePosNet3D(nn.Module):
     @torch.no_grad()
     def sample_diffusion(self, protein_pos, protein_v, batch_protein, init_ligand_pos, init_ligand_v, batch_ligand,
                          num_steps=None, center_pos_mode=None, pos_only=False, noise_tape=None, seed=None, return_traj=True,
-                         stack_traj=False, fixed_mask=None, fixed_noise_tape=None, time_seq=None):
+                         stack_traj=False, fixed_mask=None, fixed_noise_tape=None, time_seq=None, start_time=None, start_noise_tape=None):
         """The reverse-diffusion chain (reference models/molopt_score_model.py:633-703), executed entirely by libtdiff.so.
 
         Extensions over the reference signature (all optional): `noise_tape=(pos_noise [S,Nl,3], v_uniform [S,Nl,K])`
@@ -391,9 +398,26 @@ class ScorePosNet3D(nn.Module):
         Respaced sampling (DESIGN.md section 1): `time_seq` = tau_0 > ... > tau_{S-1} >= 0 with tau_0 = T - 1 runs S steps; step s
         evaluates the network at tau_s and moves the state to tau_{s+1} (to tau_{S-1} - 1 at the last step) with the exact jump
         posteriors.  `num_steps`, if given, must be S; tapes are [S, ...] (fixed tape [S+1, ...]) and trajectories [S, ...].
-        `sampling.respaced_time_seq(T, n)` makes an evenly spaced one.  Sample quality at fewer steps is not measured."""
+        `sampling.respaced_time_seq(T, n)` makes an evenly spaced one.  Sample quality at fewer steps is not measured.
+
+        Start-ligand sampling (DESIGN.md section 1): with `start_time` = t0 in 0..T-1, `init_ligand_pos` / `init_ligand_v` are a clean
+        start ligand; before the first step every row that is not fixed is replaced by a sample of q(x_t0 | x0), q(v_t0 | v0) (the types
+        are kept with pos_only), fixed rows get their sample at t0, and the chain runs from t0: `time_seq` defaults to t0, t0 - 1, ..., 0
+        (t0 + 1 steps) and must begin at t0.  `start_noise_tape=(pos_noise [Nl,3], v_uniform [Nl,K])` replaces the start draw (v_uniform
+        may be None with pos_only); it is required with `noise_tape` and not allowed without it.  Sample quality is not measured."""
+        T = self.num_timesteps
+        if start_time is not None:
+            t0 = int(start_time)
+            if not 0 <= t0 <= T - 1:
+                raise ValueError('start_time %d outside 0..T-1 = %d' % (t0, T - 1))
+            if time_seq is None:
+                time_seq = list(range(t0, -1, -1))
+            if (start_noise_tape is None) != (noise_tape is None):
+                raise ValueError('start_noise_tape is required with noise_tape, and not allowed without it')
+        elif start_noise_tape is not None:
+            raise ValueError('start_noise_tape without start_time')
         if time_seq is not None:
-            time_seq = check_time_seq(time_seq, self.num_timesteps)
+            time_seq = check_time_seq(time_seq, T, start=start_time)
             if num_steps is not None and int(num_steps) != len(time_seq):
                 raise ValueError('num_steps=%d disagrees with a time_seq of %d steps' % (int(num_steps), len(time_seq)))
             num_steps = len(time_seq)
@@ -434,6 +458,17 @@ class ScorePosNet3D(nn.Module):
             _lib.check(lib.tdiff_set_fixed_tape(eng, _ptr(fix_pn), _ptr(fix_vu)))
         elif fixed_noise_tape is not None:
             raise ValueError('fixed_noise_tape without fixed_mask')
+        if start_time is not None:
+            st_pn = st_vu = None
+            if start_noise_tape is not None:
+                st_pn = start_noise_tape[0].detach().to(dev, torch.float32).contiguous()
+                if tuple(st_pn.shape) != (Nl, 3):
+                    raise ValueError('start noise tape positions must be [Nl,3] = %s, got %s' % ((Nl, 3), tuple(st_pn.shape)))
+                if not pos_only:
+                    st_vu = start_noise_tape[1].detach().to(dev, torch.float32).contiguous()
+                    if tuple(st_vu.shape) != (Nl, K):
+                        raise ValueError('start noise tape uniforms must be [Nl,K] = %s, got %s' % ((Nl, K), tuple(st_vu.shape)))
+            _lib.check(lib.tdiff_set_start(eng, int(start_time), _ptr(st_pn), _ptr(st_vu)))
         if seed is None:        # with a tape the Philox key is unused: do not advance the caller's CPU generator (rng='cpu' driver parity)
             seed = 0 if noise_tape is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
         pos_traj = v_traj = v0_traj = vt_traj = None
