@@ -94,7 +94,14 @@ TDIFF_API const char* tdiff_version(void);
  * Replaces: Batch.from_data_list(...).to(device) + center_pos + the step-invariant half of forward
  * (scripts/sample_diffusion.py:42, models/molopt_score_model.py:110-120,333-347).
  * h_protein_counts / h_ligand_counts: atoms per graph [n_graphs].  d_protein_pos [Np,3], d_protein_feat [Np,F] fp32.
- * center_mode: 0 'none', 1 'protein' (subtract the per-graph protein centroid; scatter_mean semantics). */
+ * center_mode: 0 'none', 1 'protein' (subtract the per-graph protein centroid; scatter_mean semantics).
+ * State across calls: a bind clears the ligand state, the fixed set and its tape, the start and its tapes, and every cache of the
+ * previous batch, and sets the time (tdiff_set_time) to 0; a refused bind (TDIFF_EINVAL) changes nothing, and the batch bound before
+ * stays usable.  tdiff_set_ligand replaces the ligand state; a chain advances it and leaves the time at its last step's; tdiff_forward
+ * reads both and changes neither.  The fixed set, the start and the borrowed
+ * tapes persist across chains and tdiff_set_ligand until they are cleared or the next bind.  The caches (the previous forward's graph
+ * and edge gates, the ligand-free features built by the first chain, the protein-only neighbour keys) are exact: a call gives the same
+ * bits on a reused engine as on a fresh one bound to the same batch and given the same ligand state. */
 TDIFF_API int tdiff_bind_batch(tdiff_engine* e, int n_graphs, const int32_t* h_protein_counts, const int32_t* h_ligand_counts,
                      const float* d_protein_pos, const float* d_protein_feat, int center_mode, void* stream);
 
@@ -154,7 +161,8 @@ TDIFF_API int tdiff_sample(tdiff_engine* e, int num_steps, const float* d_pos_no
  * q_v_pred(log_onehot(v0_f)).  d_pos_traj / d_v_traj record the state after the overwrite, d_v0_traj / d_vt_traj what the network and
  * the posterior produced.  With pos_only the types of every row are left as they are.  tdiff_forward and the other calls ignore it.
  * d_mask [Nl] uint8, or NULL to clear the set; d_pos0 [Nl,3] fp32 (lab frame if apply_center != 0, centred otherwise) and d_v0 [Nl]
- * int64 are read at masked rows only (class >= num_classes -> TDIFF_EINVAL; synchronises the stream).  Before tdiff_bind_batch ->
+ * int64 are read at masked rows only (class >= num_classes -> TDIFF_EINVAL and no fixed set, until a valid call sets one; synchronises
+ * the stream).  Before tdiff_bind_batch ->
  * TDIFF_ESTATE; tdiff_bind_batch clears the set.  Costs one extra launch per chain and none per step.
  * Noise: without tapes, draw d (d = 0 before the first step, d = j + 1 after step j) comes from the same Philox key as the sampler
  * on its own counters (a, d, 0, 0x66787073) for positions and (a, d, 1 + c/4, 0x66787476) for class c; the free atoms' stream is
@@ -188,9 +196,11 @@ TDIFF_API int tdiff_sample_seq(tdiff_engine* e, const int32_t* h_time_seq, int n
                                uint64_t seed, float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only,
                                void* stream);
 
-/* Start-ligand sampling (an extension beyond the reference, DESIGN.md section 1): arms the next chains to start from the ligand state
- * set by tdiff_set_ligand (the start ligand x0, v0, centred like any ligand) noised to the start time t_start in 0..T-1, and to run
- * the reverse chain from there; t_start = -1 clears it.  While a start is armed:
+/* Start-ligand sampling (an extension beyond the reference, DESIGN.md section 1): arms the next chains to start from the current ligand
+ * state (the start ligand x0, v0, centred like any ligand) noised to the start time t_start in 0..T-1, and to run the reverse chain
+ * from there; t_start = -1 clears it.  The current ligand state is the one tdiff_set_ligand set or, after a chain, that chain's
+ * output: a second chain without tdiff_set_ligand in between re-noises the first chain's result, not the start ligand.  Set the
+ * start ligand again before each chain to draw several samples from it.  While a start is armed:
  *   the chain runs through tdiff_sample_seq only, and its time sequence must begin at tau_0 = t_start (the unit sequence
  *   t_start, ..., 0 has t_start + 1 steps; a respaced one is allowed); tdiff_sample -> TDIFF_EINVAL.  Without a start
  *   tdiff_sample_seq keeps requiring tau_0 = T - 1.

@@ -49,9 +49,14 @@ struct DevBuf {
     if (cudaMalloc(&p, want) != cudaSuccess) { (void)cudaGetLastError(); if (cudaMalloc(&p, bytes) != cudaSuccess) { (void)cudaGetLastError(); return -1; } want = bytes; }
     cap = want;
     // test switch: fill fresh allocations with 0xFF (NaN floats, negative ints) so that a read of never-written memory shows up in
-    // the parity tests instead of depending on what the allocator returns (the GPU test-suite runs with it, tests/conftest.py)
+    // the parity tests instead of depending on what the allocator returns (the GPU test-suite runs with it, tests/conftest.py).
+    // cudaMemset runs on the legacy default stream, which a non-blocking caller stream (a torch side stream) is not ordered after:
+    // wait for the fill here, so that it can never land on top of what the caller's stream writes into the buffer next
     static const bool poison = getenv("TDIFF_POISON") != nullptr;
-    if (poison) cudaMemset(p, 0xFF, want);
+    if (poison) {
+      cudaMemset(p, 0xFF, want);
+      cudaDeviceSynchronize();
+    }
     return 0;
   }
   void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
@@ -644,6 +649,9 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   }
   N = Np + Nl;
   if (N <= 0) return set_err(TDIFF_EINVAL, "empty batch");
+  // slots per row of this batch; a refused bind must leave the bound batch as it was, so nothing of `e` changes before the last
+  // refusal below
+  int K = e->KQ;
   if (e->hybrid) {
     // reference models/common.py:165-212: a ligand destination has (n_ligand - 1) ligand neighbours + k protein neighbours (torch.topk
     // raises when a graph has fewer than k protein atoms); the slot rows are sized for the largest ligand of the batch
@@ -653,15 +661,14 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
       if (lc[g] > 0 && pc[g] < e->KQ)
         return set_err(TDIFF_EINVAL, "cutoff_mode 'hybrid': graph %d has %d protein atoms < k = %d (torch.topk fails in the reference too)", g, pc[g], e->KQ);
     }
-    const int need = e->KQ + (max_lc > 0 ? max_lc - 1 : 0);
-    if (need > TD_KMAX)
+    K = e->KQ + (max_lc > 0 ? max_lc - 1 : 0);
+    if (K > TD_KMAX)
       return set_err(TDIFF_EINVAL, "cutoff_mode 'hybrid': k + n_ligand - 1 = %d + %d - 1 exceeds the %d neighbour slots per node", e->KQ, max_lc, TD_KMAX);
-    e->K = need;
   }
-  if (N * (long long)e->K >= (1LL << 31) / 1) return set_err(TDIFF_EINVAL, "batch too large: N*k = %lld edge slots", N * e->K);
+  if (N * (long long)K >= (1LL << 31) / 1) return set_err(TDIFF_EINVAL, "batch too large: N*k = %lld edge slots", N * K);
   if (max_ng > 2800) return set_err(TDIFF_EINVAL, "graph with %d nodes exceeds the k-NN kernel's shared-memory tile (2800)", max_ng);
   if (Np > 0 && (!d_ppos || !d_pfeat)) return set_err(TDIFF_EINVAL, "null protein arrays");
-  const int K = e->K;
+  e->K = K;     // the first change to `e`: every refusal is above
   std::vector<int> node_ptr(B + 1), prot_ptr(B + 1), prot_node(Np), prot_graph(Np), lig_node(Nl), lig_graph(Nl), node_lig(N, -1);
   int n = 0, p = 0, a = 0;
   for (int g = 0; g < B; ++g) {
