@@ -216,6 +216,31 @@ TDIFF_API int tdiff_sample_seq(tdiff_engine* e, const int32_t* h_time_seq, int n
  * t_start outside -1..T-1 -> TDIFF_EINVAL; tdiff_bind_batch clears the start. */
 TDIFF_API int tdiff_set_start(tdiff_engine* e, int t_start, const float* d_pos_noise, const float* d_v_uniform);
 
+/* Likelihood scoring (the variational bound of scripts/likelihood_est_diffusion.py, batched over graphs; DESIGN.md section 1).  The
+ * current ligand state is the clean ligand (x0, v0); bind with center_mode 1 ('protein') as the reference's likelihood_estimation does.
+ * Graph g is scored at h_time_steps[g] = t_g in 0..T-1 (host memory):
+ *   x_t = sqrt(abar) x0 + sqrt(1 - abar) eps, abar = alphas_cumprod[t_g], each product and the sum rounded once, and v_t by Gumbel-max
+ *   over q_v_pred(log_onehot(v0), t_g) -- the formulas and guards of the fixed set's and the start's draws;
+ *   the forward (fix_x = 0) on (x_t, v_t), a time embedding seeing t_g / T divided in fp32;
+ *   per ligand atom, the reference's terms (models/molopt_score_model.py:588-617): positions KL(q(x_{t-1} | x_t, x0) || p) / log 2 for
+ *   t_g > 0 and the decoder NLL (in nats) at t_g = 0; types categorical_kl(log_true, log_model) for t_g > 0 and
+ *   -log_categorical(log_onehot(v0), log_model) at t_g = 0; and the prior terms at T - 1 (kl_pos_prior, kl_v_prior, :411-438) with the
+ *   ligand's own types, for every graph;
+ *   per graph, the mean of each term over its ligand atoms (summed in atom order in fp32; 0 for a graph without ligand atoms).
+ * Outputs (device, each may be NULL): d_kl_pos, d_kl_v, d_prior_pos, d_prior_v [B]; d_atom_kl_pos, d_atom_kl_v [Nl]; d_xt [Nl,3]
+ * (centred frame) and d_vt [Nl] int64, the sampled state.  The ligand state is restored to x0, v0; the time embedding is left at t_g / T;
+ * the call's forward is the most recent one for tdiff_num_edges / tdiff_get_edge_index (the graph of x_t).  The fixed set and an armed
+ * start are ignored, as tdiff_forward ignores them.
+ * Noise: without a tape, atom j (its index within graph g) draws from the sampler's Philox key on counters (j, k_g, t_g << 8, 0x6c6b7073
+ * "lkps") for positions and (j, k_g, t_g << 8 | (1 + c/4), 0x6c6b7476 "lktv") for class c, so that a graph's draws, and with them its
+ * terms, do not depend on the rest of the batch.  h_keys [B] gives k_g (host memory; NULL: k_g = g).  d_pos_noise [Nl,3] and
+ * d_v_uniform [Nl,K] replace the draws (both or neither).  Launches: the forward's plus 2.  No host synchronisation beyond the pageable
+ * H2D copy of t_g and k_g.  Before bind or set_ligand -> TDIFF_ESTATE; a t_g outside 0..T-1, one half of the tape, or an engine with
+ * model_mean_type 1 ('noise', for which the reference raises) -> TDIFF_EINVAL. */
+TDIFF_API int tdiff_likelihood_terms(tdiff_engine* e, const int32_t* h_time_steps, const uint32_t* h_keys, const float* d_pos_noise,
+                                     const float* d_v_uniform, uint64_t seed, float* d_kl_pos, float* d_kl_v, float* d_prior_pos,
+                                     float* d_prior_v, float* d_atom_kl_pos, float* d_atom_kl_v, float* d_xt, int64_t* d_vt, void* stream);
+
 /* Same loop through HOST buffers (the end-to-end path: H2D of the inputs, the chain, D2H of the results, all on
  * `stream`, synchronised before returning).  Equivalent of the device-facing part of sample_diffusion_ligand
  * (scripts/sample_diffusion.py:42-112) for one batch.  h_out_* may be NULL. */

@@ -15,6 +15,14 @@
         (reference scripts/sample_diffusion.py:118-186 + scripts/batch_sample_diffusion.sh: pocket i -> `result_{i}.pt`, pockets
         assigned to workers round-robin; here the workers are the ranks of one torchrun job, one weight broadcast, no other collective)
 
+    python -m targetdiff_b200.cli score_ligands configs/sampling.yml (--pdb_path P --ligand FILE [FILE ...] | --samples RESULT.pt)
+            [--time_steps N|all] [--batch_size B] [--embedding] [--result_path DIR] [--device D]
+        (reference scripts/likelihood_est_diffusion.py: the variational-bound NLL of each ligand, targetdiff_b200.likelihood.ligand_nll;
+        --ligand files as --fragment's, in the --pdb_path pocket; --samples scores every molecule of a sample.pt / result_{i}.pt in its
+        own 'data' pocket.  Seeded by sample.seed.  Writes <result_path>/scores.pt: one dict per ligand in input order with 'kl_pos',
+        'kl_v' [n_t + 1] (the last entry the prior), 'nll', with --embedding 'pred_ligand_v', 'final_h', 'final_ligand_h', and
+        'source' (plus 'sample_index' with --samples))
+
 Result file: `<result_path>/sample.pt` (sample_for_pocket) or `<result_path>/result_{i}.pt` (sample_pockets) = {'data', 'pred_ligand_pos', 'pred_ligand_v', 'pred_ligand_pos_traj', 'pred_ligand_v_traj', 'time'}
 -- the schema scripts/sample_diffusion.py:175-182 writes and scripts/evaluate_diffusion.py:70-76 reads (positions float64, per-sample
 lists; trajectories [steps, atoms, 3]).  With `sample.respaced_steps: n` in the config (an extension beyond the reference) both commands
@@ -28,6 +36,7 @@ import sys
 import torch
 
 from .config import load_config, sampling_start, sampling_time_seq
+from .likelihood import likelihood_time_steps, ligand_nll
 from .pocket import pdb_to_pocket_data
 from .sampling import sample_diffusion_ligand, seed_all
 from .score_model import ScorePosNet3D
@@ -236,9 +245,59 @@ def sample_for_pocket(argv):
     print('Sample done! %d molecules, %.1f s' % (len(outputs[0]), sum(outputs[-1])))
 
 
+def score_ligands(argv):
+    ap = argparse.ArgumentParser(prog='targetdiff_b200.cli score_ligands')
+    ap.add_argument('config', type=str)
+    ap.add_argument('--pdb_path', type=str, help='the pocket of the --ligand files')
+    ap.add_argument('--ligand', type=str, nargs='+', help=".pt / .npz files with 'pos' [n,3] (lab frame) and 'v' [n]")
+    ap.add_argument('--samples', type=str, help='a sample.pt / result_{i}.pt: every molecule, in that file\'s own pocket')
+    ap.add_argument('--time_steps', type=str, default='10', help="N evenly spaced timesteps (i * T // N), or 'all' for every timestep")
+    ap.add_argument('--batch_size', type=int, default=640, help='(ligand, timestep) graphs per engine call')
+    ap.add_argument('--embedding', action='store_true', help='also store pred_ligand_v, final_h and final_ligand_h')
+    ap.add_argument('--result_path', type=str, default='./outputs_scores')
+    ap.add_argument('--device', type=str, default='cuda:0')
+    a = ap.parse_args(argv)
+    if bool(a.ligand) == bool(a.samples):
+        raise ValueError('give either --ligand FILE [FILE ...] (with --pdb_path) or --samples RESULT.pt, not both')
+    if a.ligand and not a.pdb_path:
+        raise ValueError('--ligand needs --pdb_path')
+    if a.samples and a.pdb_path:
+        raise ValueError('--samples scores in the pocket stored in the file: --pdb_path is not used with it')
+    config = load_config(a.config)
+    if a.ligand:
+        ligands = [_load_ligand_file(p, '--ligand')[1:] for p in a.ligand]
+        sources = [{'source': p} for p in a.ligand]
+        data = pdb_to_pocket_data(a.pdb_path)
+    else:
+        r = torch.load(a.samples, map_location='cpu', weights_only=False)
+        data = r['data']
+        ligands = list(zip(r['pred_ligand_pos'], r['pred_ligand_v']))
+        sources = [{'source': a.samples, 'sample_index': i} for i in range(len(ligands))]
+    seed_all(config.sample.seed)
+    seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # the likelihood stream's key, drawn before loading the model
+    model = _load_model(config, a.device)
+    if a.embedding and model.time_emb_dim > 0:
+        raise ValueError('--embedding needs a checkpoint without a time embedding (the reference fetch_embedding cannot run either)')
+    T = model.num_timesteps
+    time_steps = likelihood_time_steps(T, T if a.time_steps == 'all' else int(a.time_steps))
+    scores = ligand_nll(model, data, ligands, time_steps=time_steps, batch_size=a.batch_size, device=a.device, seed=seed,
+                        embedding=a.embedding)
+    out = []
+    for src, sc in zip(sources, scores):
+        d = {'kl_pos': sc['kl_pos'], 'kl_v': sc['kl_v'], 'nll': sc['nll']}
+        for k in ('pred_ligand_v', 'final_h', 'final_ligand_h'):
+            if k in sc:
+                d[k] = sc[k]
+        d.update(src)
+        out.append(d)
+    os.makedirs(a.result_path, exist_ok=True)
+    torch.save(out, os.path.join(a.result_path, 'scores.pt'))
+    print('Scored %d ligands at %d timesteps' % (len(out), len(time_steps)))
+
+
 def main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
-    commands = {'sample_for_pocket': sample_for_pocket, 'sample_pockets': sample_pockets}
+    commands = {'sample_for_pocket': sample_for_pocket, 'sample_pockets': sample_pockets, 'score_ligands': score_ligands}
     if not argv or argv[0] not in commands:
         raise SystemExit(__doc__)
     commands[argv[0]](argv[1:])

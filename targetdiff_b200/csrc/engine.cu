@@ -136,6 +136,9 @@ struct tdiff_engine {
   // log_alphas_v[i]; the per-step tables of the current chain: seq_t, seq_p [S] int | c0, ct, logvar, la, l1ma [S] fp32
   std::vector<double> cum_log_a, cum_log_av;
   DevBuf seq_buf;
+  // likelihood scoring (tdiff_likelihood_terms): t_g, k_g [B] int32 | the clean ligand x0 [Nl] float4, v0 [Nl] int, kept during the call
+  DevBuf lk_buf, lk_x0, lk_v0;
+  std::vector<int32_t> lk_host;
   DevBuf stage[8];   // staging for tdiff_sample_host
   // ---- instrumentation
   cudaStream_t own_stream = nullptr;   // capture stream (the caller's stream may be the legacy default stream, which cannot capture)
@@ -625,7 +628,7 @@ extern "C" void tdiff_destroy(tdiff_engine* e) {
   if (e->ev_join) cudaEventDestroy(e->ev_join);
   DevBuf* bufs[] = {&e->node_ptr, &e->prot_ptr, &e->prot_node, &e->prot_graph, &e->lig_node, &e->lig_graph, &e->node_lig, &e->xm0, &e->xm1,
                     &e->rel_flag, &e->rel_list, &e->n_rel, &e->work_list, &e->n_work, &e->knn_cache, &e->x2h_rows, &e->lig_rows, &e->rel_rows, &e->rel_counts, &e->ew_x2h, &e->ew_h2x, &e->h_sync, &e->hagg, &e->time_norm, &e->h_free, &e->dirty, &e->free_rows, &e->free_counts, &e->lig_save, &e->offset, &e->h0, &e->h, &e->P, &e->q, &e->src, &e->src_prev, &e->etype, &e->e_w, &e->dist, &e->kbuf, &e->vbuf, &e->v16, &e->lig_pos,
-                    &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges, &e->fix_mask, &e->fix_pos, &e->fix_v, &e->seq_buf};
+                    &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges, &e->fix_mask, &e->fix_pos, &e->fix_v, &e->seq_buf, &e->lk_buf, &e->lk_x0, &e->lk_v0};
   for (auto* b : bufs) b->release();
   for (auto& b : e->stage) b.release();
   if (e->arena) cudaFree(e->arena);
@@ -1375,6 +1378,61 @@ extern "C" int tdiff_sample_seq(tdiff_engine* e, const int32_t* h_time_seq, int 
                                 void* stream) {
   if (!h_time_seq) return set_err(TDIFF_EINVAL, "time sequence: null pointer");
   return sample_chain(e, h_time_seq, num_steps, d_pos_noise, d_v_uniform, seed, d_pos_traj, d_v_traj, d_v0_traj, d_vt_traj, pos_only, stream);
+}
+
+// Likelihood scoring (DESIGN.md section 1): one init launch (x0 / v0 saved, x_t / v_t drawn, t_g / T), the forward, one epilogue launch
+// (per-atom terms, per-graph means, x0 / v0 restored).  The only host-side wait is the pageable H2D copy of t_g, k_g.
+extern "C" int tdiff_likelihood_terms(tdiff_engine* e, const int32_t* h_time_steps, const uint32_t* h_keys, const float* d_pos_noise,
+                                      const float* d_v_uniform, uint64_t seed, float* d_kl_pos, float* d_kl_v, float* d_prior_pos,
+                                      float* d_prior_v, float* d_atom_kl_pos, float* d_atom_kl_v, float* d_xt, int64_t* d_vt, void* stream) {
+  if (!e || !e->bound || !e->has_ligand) return set_err(TDIFF_ESTATE, "likelihood_terms needs bind_batch + set_ligand first");
+  const int T = e->cfg.num_timesteps, B = e->B;
+  if (!h_time_steps) return set_err(TDIFF_EINVAL, "likelihood_terms: null time steps");
+  if (e->cfg.model_mean_type != 0)
+    return set_err(TDIFF_EINVAL, "likelihood_terms needs model_mean_type C0 (the reference raises for 'noise' too)");
+  if (T >= (1 << 24)) return set_err(TDIFF_EINVAL, "likelihood_terms: T = %d does not fit the stream's 24-bit time field", T);
+  for (int g = 0; g < B; ++g)
+    if (h_time_steps[g] < 0 || h_time_steps[g] > T - 1)
+      return set_err(TDIFF_EINVAL, "likelihood_terms: time step %d of graph %d outside 0..%d", h_time_steps[g], g, T - 1);
+  if ((d_pos_noise == nullptr) != (d_v_uniform == nullptr))
+    return set_err(TDIFF_EINVAL, "likelihood_terms: the tape needs both pos_noise and v_uniform (or neither for Philox)");
+  cudaStream_t st = (cudaStream_t)stream;
+  CK(cudaSetDevice(e->device));
+  const size_t Nl = (size_t)e->Nl;
+  if (e->lk_buf.ensure((size_t)B * 8 + 16) | e->lk_x0.ensure(Nl * 16 + 16) | e->lk_v0.ensure(Nl * 4 + 16))
+    return set_err(TDIFF_ECUDA, "out of device memory for likelihood scoring of %d graphs", B);
+  e->lk_host.resize(2 * (size_t)B);
+  for (int g = 0; g < B; ++g) {
+    e->lk_host[g] = h_time_steps[g];
+    e->lk_host[B + g] = (int32_t)(h_keys ? h_keys[g] : (uint32_t)g);
+  }
+  CK(cudaMemcpyAsync(e->lk_buf.p, e->lk_host.data(), (size_t)B * 8, cudaMemcpyHostToDevice, st));
+  TdLikelihoodArgs L;
+  memset(&L, 0, sizeof(L));
+  TdStepArgs& A = L.A;
+  A.n_lig = e->Nl; A.n_classes = e->cfg.num_classes; A.pos_only = 0; A.seed = seed;
+  A.lig_graph = e->lig_graph.as<int>(); A.lig_pos = e->lig_pos.as<float4>(); A.lig_v = e->lig_v.as<int>();
+  A.ac = e->t_ac; A.lca_v = e->t_lca; A.l1mca_v = e->t_l1mca; A.log_k = (float)log((double)e->cfg.num_classes);
+  A.lk_t = e->lk_buf.as<int>(); A.lk_key = (const unsigned*)(e->lk_buf.as<int>() + B);
+  A.lk_pos_noise = d_pos_noise; A.lk_v_uniform = d_v_uniform;
+  L.n_graphs = B; L.n_timesteps = T;
+  L.node_ptr = e->node_ptr.as<int>(); L.prot_ptr = e->prot_ptr.as<int>(); L.lig_node = e->lig_node.as<int>();
+  L.logits = e->logits.as<float>();
+  L.c0 = e->t_c0; L.ct = e->t_ct; L.logvar = e->t_logvar; L.la_v = e->t_la; L.l1ma_v = e->t_l1ma;
+  L.x0 = e->lk_x0.as<float4>(); L.v0 = e->lk_v0.as<int>();
+  L.time_norm = e->time_emb ? e->time_norm.as<float>() : nullptr;
+  L.kl_pos = d_kl_pos; L.kl_v = d_kl_v; L.prior_pos = d_prior_pos; L.prior_v = d_prior_v;
+  L.atom_kl_pos = d_atom_kl_pos; L.atom_kl_v = d_atom_kl_v; L.xt = d_xt; L.vt = (long long*)d_vt;
+  td_launch_likelihood_init(L, st);
+  e->launches += 1;
+  Prof* total = new Prof(e, st, EV_TOTAL);
+  run_forward(e, st, 0);
+  delete total;
+  L.xm_final = e->final_buf ? e->xm1.as<float4>() : e->xm0.as<float4>();
+  td_launch_likelihood_epilogue(L, st);
+  e->launches += 1;
+  CK(cudaGetLastError());
+  return TDIFF_OK;
 }
 
 extern "C" int tdiff_sample_host(tdiff_engine* e, int B, const int32_t* pc, const int32_t* lc, const float* h_ppos, const float* h_pfeat,

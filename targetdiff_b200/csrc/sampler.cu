@@ -35,24 +35,51 @@ __device__ __forceinline__ float log_add_exp_f(float a, float b) {
 #define TD_START_POS_DOMAIN 0x73747073u
 #define TD_START_TYPE_DOMAIN 0x73747476u
 
+// Philox domain words of the likelihood stream ("lkps", "lktv"), distinct from the six above (oracle/likelihood.py)
+#define TD_LK_POS_DOMAIN 0x6c6b7073u
+#define TD_LK_TYPE_DOMAIN 0x6c6b7476u
+
+// Draw layout of forward_sample: tape row `d * Nl + a` and Philox counter (a, d, lane, domain), lane 0 for positions and 1 + c/4 for
+// class c -- the fixed-atom and start streams'
+struct TdDrawByRow {
+  static __device__ __forceinline__ size_t row(const TdStepArgs& A, int a, int d) { return (size_t)d * A.n_lig + a; }
+  static __device__ __forceinline__ uint4 counter(const TdStepArgs&, int a, int d, unsigned lane, unsigned domain) {
+    return make_uint4((unsigned)a, (unsigned)d, lane, domain);
+  }
+};
+
 // Sources of forward_sample: x0 / v0, the tapes and the Philox domain words of the fixed-atom stream and of the start stream
-struct TdFixedSource {
+struct TdFixedSource : TdDrawByRow {
   static constexpr unsigned kPosDomain = TD_FIX_POS_DOMAIN, kTypeDomain = TD_FIX_TYPE_DOMAIN;
   static __device__ __forceinline__ const float4* x0(const TdStepArgs& A) { return A.fix_pos; }
   static __device__ __forceinline__ const int* v0(const TdStepArgs& A) { return A.fix_v; }
   static __device__ __forceinline__ const float* pos_tape(const TdStepArgs& A) { return A.fix_pos_noise; }
   static __device__ __forceinline__ const float* v_tape(const TdStepArgs& A) { return A.fix_v_uniform; }
 };
-struct TdStartSource {            // the start ligand is the chain's own state before the start draw
+struct TdStartSource : TdDrawByRow {   // the start ligand is the chain's own state before the start draw
   static constexpr unsigned kPosDomain = TD_START_POS_DOMAIN, kTypeDomain = TD_START_TYPE_DOMAIN;
   static __device__ __forceinline__ const float4* x0(const TdStepArgs& A) { return A.lig_pos; }
   static __device__ __forceinline__ const int* v0(const TdStepArgs& A) { return A.lig_v; }
   static __device__ __forceinline__ const float* pos_tape(const TdStepArgs& A) { return A.start_pos_noise; }
   static __device__ __forceinline__ const float* v_tape(const TdStepArgs& A) { return A.start_v_uniform; }
 };
+// Likelihood scoring: the clean ligand is the ligand state; `d` is the atom's index j within its graph g, so that the counter
+// (j, k_g, t_g << 8 | lane, domain) does not depend on where the graph sits in the batch.  The tape is [Nl, .] in batch order.
+struct TdLikelihoodSource {
+  static constexpr unsigned kPosDomain = TD_LK_POS_DOMAIN, kTypeDomain = TD_LK_TYPE_DOMAIN;
+  static __device__ __forceinline__ const float4* x0(const TdStepArgs& A) { return A.lig_pos; }
+  static __device__ __forceinline__ const int* v0(const TdStepArgs& A) { return A.lig_v; }
+  static __device__ __forceinline__ const float* pos_tape(const TdStepArgs& A) { return A.lk_pos_noise; }
+  static __device__ __forceinline__ const float* v_tape(const TdStepArgs& A) { return A.lk_v_uniform; }
+  static __device__ __forceinline__ size_t row(const TdStepArgs&, int a, int) { return (size_t)a; }
+  static __device__ __forceinline__ uint4 counter(const TdStepArgs& A, int a, int d, unsigned lane, unsigned domain) {
+    const int g = A.lig_graph[a];
+    return make_uint4((unsigned)d, A.lk_key[g], ((unsigned)A.lk_t[g] << 8) | lane, domain);
+  }
+};
 
-// Row `a`: a sample of q(x_tm | x0) and q(v_tm | v0) with x0 / v0 from `Src`, from draw `d` of its stream (the sampler's key and counter
-// layout on Src's domain words) or rows d of its tapes [., Nl, 3] / [., Nl, K]; x0 / v0 exactly when tm < 0.  Position
+// Row `a`: a sample of q(x_tm | x0) and q(v_tm | v0) with x0 / v0 from `Src`, from draw `d` of its stream (the sampler's key, Src's
+// counter layout and domain words) or row Src::row(a, d) of its tapes [., 3] / [., K]; x0 / v0 exactly when tm < 0.  Position
 // sqrt(ac) x0 + sqrt(1 - ac) eps with every product and the sum rounded once, as the reference's perturbation
 // (models/molopt_score_model.py:500-504); type: Gumbel-max over the unnormalised q_v_pred(log_onehot(v0), tm) (q_v_sample, :394-398).
 // With pos_only the type is left as it is.
@@ -67,10 +94,10 @@ __device__ __forceinline__ void forward_sample(const TdStepArgs& A, int a, int d
   const uint2 key = make_uint2((unsigned)A.seed, (unsigned)(A.seed >> 32));
   float nz[3];
   if (Src::pos_tape(A)) {
-    const float* pn = Src::pos_tape(A) + ((size_t)d * A.n_lig + a) * 3;
+    const float* pn = Src::pos_tape(A) + Src::row(A, a, d) * 3;
     nz[0] = pn[0]; nz[1] = pn[1]; nz[2] = pn[2];
   } else {
-    const uint4 r0 = philox4x32_10(make_uint4((unsigned)a, (unsigned)d, 0u, Src::kPosDomain), key);
+    const uint4 r0 = philox4x32_10(Src::counter(A, a, d, 0u, Src::kPosDomain), key);
     const float u0 = 1.0f - u01(r0.x), u1 = u01(r0.y), u2 = 1.0f - u01(r0.z), u3 = u01(r0.w);
     const float ra = sqrtf(-2.0f * logf(u0)), rb = sqrtf(-2.0f * logf(u2));
     nz[0] = ra * cospif(2.0f * u1); nz[1] = ra * sinpif(2.0f * u1); nz[2] = rb * cospif(2.0f * u3);
@@ -90,10 +117,10 @@ __device__ __forceinline__ void forward_sample(const TdStepArgs& A, int a, int d
   for (int c0 = 0; c0 < K; c0 += 4) {
     float u[4];
     if (Src::v_tape(A)) {
-      const float* vu = Src::v_tape(A) + ((size_t)d * A.n_lig + a) * K;
+      const float* vu = Src::v_tape(A) + Src::row(A, a, d) * K;
       for (int j = 0; j < 4 && c0 + j < K; ++j) u[j] = vu[c0 + j];
     } else {
-      const uint4 r = philox4x32_10(make_uint4((unsigned)a, (unsigned)d, 1u + (unsigned)(c0 >> 2), Src::kTypeDomain), key);
+      const uint4 r = philox4x32_10(Src::counter(A, a, d, 1u + (unsigned)(c0 >> 2), Src::kTypeDomain), key);
       u[0] = u01(r.x); u[1] = u01(r.y); u[2] = u01(r.z); u[3] = u01(r.w);
     }
     for (int j = 0; j < 4 && c0 + j < K; ++j) {
@@ -271,6 +298,142 @@ __global__ void start_init_kernel(TdStepArgs A) {
 }
 void td_launch_start_init(const TdStepArgs& A, cudaStream_t st) {
   if (A.n_lig > 0) start_init_kernel<<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
+}
+
+// ---------------------------------------------------------------------------------------- likelihood scoring
+// tdiff_likelihood_terms (DESIGN.md section 1): graph g at t_g.  Before the forward: x0 / v0 saved to scratch, every row <- a sample of
+// q(x_t | x0), q(v_t | v0) at t_g (forward_sample on the likelihood stream or tape), time_norm[g] = t_g / T divided in fp32.
+__global__ void likelihood_init_kernel(TdLikelihoodArgs L) {
+  const TdStepArgs& A = L.A;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (L.time_norm && i < L.n_graphs) L.time_norm[i] = __fdiv_rn((float)A.lk_t[i], (float)L.n_timesteps);
+  if (i >= A.n_lig) return;
+  const int g = A.lig_graph[i];
+  const int j = i - (L.node_ptr[g] - L.prot_ptr[g]);
+  L.x0[i] = A.lig_pos[i];
+  L.v0[i] = A.lig_v[i];
+  float4 x;
+  int v = A.lig_v[i];
+  forward_sample<TdLikelihoodSource>(A, i, j, A.lk_t[g], x, v);
+  A.lig_pos[i] = x;
+  A.lig_v[i] = v;
+}
+void td_launch_likelihood_init(const TdLikelihoodArgs& L, cudaStream_t st) {
+  const int n = L.A.n_lig > L.n_graphs ? L.A.n_lig : L.n_graphs;
+  if (n > 0) likelihood_init_kernel<<<(n + 127) / 128, 128, 0, st>>>(L);
+}
+
+// After the forward: the per-atom terms of graph g, restated op by op from the reference (models/molopt_score_model.py:133-155
+// normal_kl / log_normal / categorical_kl / log_categorical, :401-409 q_v_posterior, :411-438 the priors, :470-489 compute_pos_Lt /
+// compute_v_Lt, :588-617 likelihood_estimation), their means over the graph's ligand atoms (summed in atom order in fp32, then divided
+// by the count, as scatter_mean on CPU; 0 for a graph without ligand atoms), and the ligand state restored to x0 / v0.  One block per
+// graph: each chunk of 128 atoms puts its terms in shared memory and thread 0 adds them up in order.
+__global__ void __launch_bounds__(128) likelihood_epilogue_kernel(TdLikelihoodArgs L) {
+  const TdStepArgs& A = L.A;
+  __shared__ float terms[4][128];
+  const int g = blockIdx.x, tid = threadIdx.x;
+  const int b = L.node_ptr[g] - L.prot_ptr[g], e = L.node_ptr[g + 1] - L.prot_ptr[g + 1];
+  const int t = A.lk_t[g], T = L.n_timesteps, K = A.n_classes;
+  const float log_eps = -69.07755279f;                                     // logf(1e-30f): index_to_log_onehot's clamp
+  const float log_sqrt_2pi = 0.918938533f;                                 // np.log(np.sqrt(2 * np.pi)) in fp32
+  const float log_2 = 0.693147181f;                                        // np.log(2.) in fp32
+  float sum[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int base = b; base < e; base += 128) {
+    const int a = base + tid;
+    if (a < e) {
+      const float4 x0 = L.x0[a], xt = A.lig_pos[a], px = L.xm_final[L.lig_node[a]];
+      const int v0 = L.v0[a], vt = A.lig_v[a];
+      const float x0v[3] = {x0.x, x0.y, x0.z}, xtv[3] = {xt.x, xt.y, xt.z}, pxv[3] = {px.x, px.y, px.z};
+      // ---- positions: q_pos_posterior of the model's x0 and of the true x0, each product and sum rounded once (:424-428)
+      const float c0 = L.c0[t], ct = L.ct[t], lv = L.logvar[t];
+      float tp = 0.f;
+      if (t > 0) {                 // normal_kl(mean_true, lv, mean_model, lv) / log 2 (compute_pos_Lt, :470-482)
+        for (int d = 0; d < 3; ++d) {
+          const float ctx = __fmul_rn(ct, xtv[d]);
+          const float df = __fadd_rn(__fmul_rn(c0, x0v[d]), ctx) - __fadd_rn(__fmul_rn(c0, pxv[d]), ctx);
+          tp += 0.5f * ((((-1.0f + lv) - lv) + expf(lv - lv)) + __fmul_rn(__fmul_rn(df, df), expf(-lv)));
+        }
+        tp = tp / log_2;
+      } else {                     // decoder: -log_normal(x0, mean_model, 0.5 lv), in nats
+        const float ls = 0.5f * lv, var2 = 2.0f * expf(ls * 2.0f);
+        float lp = 0.f;
+        for (int d = 0; d < 3; ++d) {
+          const float df = x0v[d] - __fadd_rn(__fmul_rn(c0, pxv[d]), __fmul_rn(ct, xtv[d]));
+          lp += ((-__fmul_rn(df, df)) / var2 - ls) - log_sqrt_2pi;
+        }
+        tp = -lp;
+      }
+      // ---- types: q_v_posterior of log_softmax(logits) and of log_onehot(v0) given v_t (:401-409), at t - 1 clamped to 0
+      const float* lg = L.logits + (size_t)a * K;
+      float lr[TD_CMAX], um[TD_CMAX], ut[TD_CMAX];
+      float mx = -INFINITY;
+      for (int c = 0; c < K; ++c) { lr[c] = lg[c]; mx = fmaxf(mx, lr[c]); }
+      float se = 0.0f;
+      for (int c = 0; c < K; ++c) se += expf(lr[c] - mx);
+      const float lse = logf(se);
+      for (int c = 0; c < K; ++c) lr[c] = (lr[c] - mx) - lse;
+      const int tm1 = t > 0 ? t - 1 : 0;
+      const float lca = A.lca_v[tm1], l1mca = A.l1mca_v[tm1] - A.log_k;
+      const float la = L.la_v[t], l1ma = L.l1ma_v[t] - A.log_k;
+      float mm = -INFINITY, mt = -INFINITY;
+      for (int c = 0; c < K; ++c) {
+        const float q1 = log_add_exp_f(((c == vt) ? 0.0f : log_eps) + la, l1ma);
+        um[c] = log_add_exp_f(lr[c] + lca, l1mca) + q1;
+        ut[c] = log_add_exp_f(((c == v0) ? 0.0f : log_eps) + lca, l1mca) + q1;
+        mm = fmaxf(mm, um[c]); mt = fmaxf(mt, ut[c]);
+      }
+      float sm = 0.f, st = 0.f;
+      for (int c = 0; c < K; ++c) { sm += expf(um[c] - mm); st += expf(ut[c] - mt); }
+      const float lsm = mm + logf(sm), lst = mt + logf(st);                // torch.logsumexp
+      float tv = 0.f;
+      if (t > 0) {                 // categorical_kl(log_true, log_model)
+        for (int c = 0; c < K; ++c) {
+          const float lt = ut[c] - lst;
+          tv += __fmul_rn(expf(lt), lt - (um[c] - lsm));
+        }
+      } else {                     // -log_categorical(log_onehot(v0), log_model): the clamped entries weigh exp(log 1e-30)
+        const float w_eps = expf(log_eps);
+        for (int c = 0; c < K; ++c) tv += __fmul_rn((c == v0) ? 1.0f : w_eps, um[c] - lsm);
+        tv = -tv;
+      }
+      // ---- priors at T - 1 with the ligand's own types (kl_pos_prior / kl_v_prior, :411-438)
+      const float acT = A.ac[T - 1];
+      const float sa = sqrtf(acT), lv2 = logf(sqrtf(1.0f - acT));
+      float pp = 0.f;
+      for (int d = 0; d < 3; ++d) {
+        const float m = __fmul_rn(sa, x0v[d]);
+        pp += 0.5f * ((((-1.0f + lv2) - 0.0f) + expf(0.0f - lv2)) + __fmul_rn(__fmul_rn(0.0f - m, 0.0f - m), expf(-lv2)));
+      }
+      const float lcaT = A.lca_v[T - 1], l1mcaT = A.l1mca_v[T - 1] - A.log_k, log_half = -logf((float)K);
+      float pv = 0.f;
+      for (int c = 0; c < K; ++c) {
+        const float lq = log_add_exp_f(((c == v0) ? 0.0f : log_eps) + lcaT, l1mcaT);
+        pv += __fmul_rn(expf(lq), lq - log_half);
+      }
+      terms[0][tid] = tp; terms[1][tid] = tv; terms[2][tid] = pp; terms[3][tid] = pv;
+      if (L.atom_kl_pos) L.atom_kl_pos[a] = tp;
+      if (L.atom_kl_v) L.atom_kl_v[a] = tv;
+      if (L.xt) { L.xt[3 * a] = xt.x; L.xt[3 * a + 1] = xt.y; L.xt[3 * a + 2] = xt.z; }
+      if (L.vt) L.vt[a] = (long long)vt;
+      A.lig_pos[a] = x0;
+      A.lig_v[a] = v0;
+    }
+    __syncthreads();
+    if (tid == 0) {
+      const int n = min(128, e - base);
+      for (int i = 0; i < n; ++i) { sum[0] += terms[0][i]; sum[1] += terms[1][i]; sum[2] += terms[2][i]; sum[3] += terms[3][i]; }
+    }
+    __syncthreads();
+  }
+  if (tid != 0) return;
+  const float cnt = (float)(e - b > 0 ? e - b : 1);
+  if (L.kl_pos) L.kl_pos[g] = sum[0] / cnt;
+  if (L.kl_v) L.kl_v[g] = sum[1] / cnt;
+  if (L.prior_pos) L.prior_pos[g] = sum[2] / cnt;
+  if (L.prior_v) L.prior_v[g] = sum[3] / cnt;
+}
+void td_launch_likelihood_epilogue(const TdLikelihoodArgs& L, cudaStream_t st) {
+  if (L.n_graphs > 0) likelihood_epilogue_kernel<<<L.n_graphs, 128, 0, st>>>(L);
 }
 
 // fixed set in (tdiff_set_fixed): positions and classes are read at masked rows only; lab frame -> centred like set_ligand_kernel

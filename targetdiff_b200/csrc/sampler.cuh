@@ -40,11 +40,37 @@ struct TdStepArgs {
   // start chain (tdiff_set_start): the start draw's tape, read by start_init_kernel only
   const float* start_pos_noise;    // [Nl,3] or NULL (Philox, START_POS domain)
   const float* start_v_uniform;    // [Nl,K] or NULL (Philox, START_TYPE domain)
+  // likelihood scoring (tdiff_likelihood_terms): per-graph timestep and draw key, the noising draw's tape; read by likelihood kernels only
+  const int* lk_t;                 // [B] t_g in 0..T-1
+  const unsigned* lk_key;          // [B] k_g
+  const float* lk_pos_noise;       // [Nl,3] or NULL (Philox, LK_POS domain)
+  const float* lk_v_uniform;       // [Nl,K] or NULL (Philox, LK_TYPE domain)
+};
+
+// likelihood scoring (DESIGN.md section 1): the noising draw (TdStepArgs A) and the epilogue's own tables and outputs
+struct TdLikelihoodArgs {
+  TdStepArgs A;                    // n_lig, n_classes, seed, ac, lca_v, l1mca_v, log_k, lig_pos, lig_v, lig_graph, lk_*
+  int n_graphs, n_timesteps;
+  const int *node_ptr, *prot_ptr;  // [B+1]: graph g's ligand atoms are node_ptr[g] - prot_ptr[g] .. node_ptr[g+1] - prot_ptr[g+1] - 1
+  const float4* xm_final;          // node array after the forward (predicted x0, centred)
+  const int* lig_node;             // [Nl]
+  const float* logits;             // [Nl,K]
+  const float *c0, *ct, *logvar;   // posterior_mean_c0_coef, posterior_mean_ct_coef, posterior_logvar [T]
+  const float *la_v, *l1ma_v;      // log_alphas_v, log_one_minus_alphas_v [T]
+  float4* x0;                      // scratch [Nl]: the clean ligand, restored into lig_pos by the epilogue
+  int* v0;                         // scratch [Nl]
+  float* time_norm;                // [B] t_g / T, or NULL (no time embedding)
+  float *kl_pos, *kl_v, *prior_pos, *prior_v;   // [B] or NULL
+  float *atom_kl_pos, *atom_kl_v;  // [Nl] or NULL
+  float* xt;                       // [Nl,3] centred x_t, or NULL
+  long long* vt;                   // [Nl] v_t, or NULL
 };
 
 void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st);
 void td_launch_fixed_init(const TdStepArgs& A, cudaStream_t st);
 void td_launch_start_init(const TdStepArgs& A, cudaStream_t st);
+void td_launch_likelihood_init(const TdLikelihoodArgs& L, cudaStream_t st);
+void td_launch_likelihood_epilogue(const TdLikelihoodArgs& L, cudaStream_t st);
 void td_launch_set_fixed(const unsigned char* mask, const float* pos, const long long* v, const int* lig_graph, const float4* offset,
                          int apply_center, int n, int n_classes, unsigned char* fix_mask, float4* fix_pos, int* fix_v, int* err,
                          cudaStream_t st);

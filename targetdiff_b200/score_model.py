@@ -580,6 +580,62 @@ class ScorePosNet3D(nn.Module):
         return kl_pos, kl_v
 
     @torch.no_grad()
+    def likelihood_terms(self, protein_pos, protein_v, batch_protein, ligand_pos, ligand_v, batch_ligand, time_step, keys=None, seed=None,
+                         noise=None, return_atoms=False):
+        """Variational-bound terms of every graph at its own `time_step` [B] (0..T-1) in one engine call (tdiff_likelihood_terms,
+        DESIGN.md section 1): noising, the forward and the per-atom terms and per-graph means on the device, plus the prior terms of
+        every graph with the ligand's own types.  The ligand is the clean one, in the lab frame; everything is centred on the protein.
+        Noise comes from the engine's likelihood stream, keyed per graph by `keys` [B] (default: the graph index) and `seed` (default:
+        drawn from torch's CPU generator), so a graph's terms do not depend on the rest of the batch; `noise=(pos_noise [Nl,3],
+        v_uniform [Nl,K])` replaces it.  Returns device tensors kl_pos, kl_v, prior_pos, prior_v [B]; `return_atoms` adds atom_kl_pos,
+        atom_kl_v [Nl], xt [Nl,3] (centred frame) and vt [Nl].  `likelihood_estimation` above stays the reference-signature entry with
+        the reference's random stream and graph-id prior."""
+        T, K = self.num_timesteps, self.num_classes
+        if self.model_mean_type != 'C0':          # the reference raises (models/molopt_score_model.py:601-605)
+            raise ValueError('likelihood_terms needs model_mean_type C0, got %r' % (self.model_mean_type,))
+        ts = [int(x) for x in torch.as_tensor(time_step).reshape(-1).tolist()]
+        if any(not 0 <= x <= T - 1 for x in ts):
+            raise ValueError('time_step must lie in 0..T-1 = %d' % (T - 1))
+        dev = protein_pos.device
+        eng = self.engine(dev)
+        lib = _lib.load()
+        st = self._stream(dev)
+        B, Np, Nl = self._bind(eng, protein_pos, protein_v, batch_protein, batch_ligand, 1)
+        if len(ts) != B:
+            raise ValueError('time_step must have one entry per graph: %d entries, %d graphs' % (len(ts), B))
+        key_arr = None
+        if keys is not None:
+            kl = [int(x) for x in torch.as_tensor(keys).reshape(-1).tolist()]
+            if len(kl) != B or any(not 0 <= x < 2 ** 32 for x in kl):
+                raise ValueError('keys must be %d integers in 0..2^32-1' % B)
+            key_arr = (ctypes.c_uint32 * B)(*kl)
+        lpos = ligand_pos.detach().to(torch.float32).contiguous()
+        lv = ligand_v.detach().to(torch.int64).contiguous()
+        if lpos.shape[0] != Nl or lv.shape[0] != Nl:
+            raise ValueError('ligand arrays disagree with batch_ligand')
+        _lib.check(lib.tdiff_set_ligand(eng, _ptr(lpos), _ptr(lv), 1, st))
+        pos_noise = v_uniform = None
+        if noise is not None:
+            pos_noise = noise[0].detach().to(dev, torch.float32).contiguous()
+            v_uniform = noise[1].detach().to(dev, torch.float32).contiguous()
+            if tuple(pos_noise.shape) != (Nl, 3) or tuple(v_uniform.shape) != (Nl, K):
+                raise ValueError('noise shapes must be [Nl,3] = %s and [Nl,K] = %s, got %s and %s'
+                                 % ((Nl, 3), (Nl, K), tuple(pos_noise.shape), tuple(v_uniform.shape)))
+        if seed is None:        # as sample_diffusion: with a tape the key is unused and the caller's CPU generator is not advanced
+            seed = 0 if noise is not None else int(torch.randint(0, 2 ** 62, (1,)).item())
+        out = {k: torch.empty(B, device=dev) for k in ('kl_pos', 'kl_v', 'prior_pos', 'prior_v')}
+        atoms = {}
+        if return_atoms:
+            atoms = {'atom_kl_pos': torch.empty(Nl, device=dev), 'atom_kl_v': torch.empty(Nl, device=dev),
+                     'xt': torch.empty(Nl, 3, device=dev), 'vt': torch.empty(Nl, dtype=torch.int64, device=dev)}
+        _lib.check(lib.tdiff_likelihood_terms(eng, _lib.i32_array(ts), key_arr, _ptr(pos_noise), _ptr(v_uniform), ctypes.c_uint64(seed),
+                                              _ptr(out['kl_pos']), _ptr(out['kl_v']), _ptr(out['prior_pos']), _ptr(out['prior_v']),
+                                              _ptr(atoms.get('atom_kl_pos')), _ptr(atoms.get('atom_kl_v')), _ptr(atoms.get('xt')),
+                                              _ptr(atoms.get('vt')), st))
+        out.update(atoms)
+        return out
+
+    @torch.no_grad()
     def fetch_embedding(self, protein_pos, protein_v, batch_protein, ligand_pos, ligand_v, batch_ligand):
         """reference models/molopt_score_model.py:619-631: forward with fix_x=True."""
         return self.forward(protein_pos, protein_v, batch_protein, ligand_pos, ligand_v, batch_ligand, fix_x=True)
