@@ -292,6 +292,12 @@ TDIFF_API int tdiff_edge_mlp_mode(tdiff_engine* e);
 TDIFF_API int tdiff_profile(tdiff_engine* e, int enable);
 TDIFF_API int tdiff_profile_read(tdiff_engine* e, double* ms_aggregate_h, int64_t* n_aggregate_h, double* ms_aggregate_x,
                        int64_t* n_aggregate_x, double* ms_edge_mlp, int64_t* n_edge_mlp, double* ms_total);
+/* Node lists of the last sampling step's backward cone (DESIGN.md section 4.3), copied to the host by synchronous copies (call once
+ * the step's stream has finished).  h_dims = {G x2h evaluations of the last block, row stride}; then, where not NULL, 2 G class-sorted
+ * lists: h_counts [2G,4] = {entries, protein part, protein nodes, -}, h_rows [2G,stride] (-1 = padding; order within a class
+ * unspecified); list 2g holds the destinations of evaluation g, list 2g+1 the nodes whose B blocks it computes.  TDIFF_ESTATE when no
+ * sampling step has built them since the batch was bound. */
+TDIFF_API int tdiff_get_cone(tdiff_engine* e, int32_t* h_dims, int32_t* h_counts, int32_t* h_rows);
 
 #ifdef __cplusplus
 }

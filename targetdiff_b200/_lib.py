@@ -66,6 +66,7 @@ SIGNATURES = {
     'tdiff_profile': (_i, [_vp, _i]),
     'tdiff_profile_read': (_i, [_vp, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(_i64), ctypes.POINTER(ctypes.c_double),
                                 ctypes.POINTER(_i64), ctypes.POINTER(ctypes.c_double), ctypes.POINTER(_i64), ctypes.POINTER(ctypes.c_double)]),
+    'tdiff_get_cone': (_i, [_vp, _vp, _vp, _vp]),
 }
 
 _lib = None

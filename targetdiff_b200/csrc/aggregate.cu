@@ -157,11 +157,13 @@ void td_launch_aggregate_x(const float* kbuf, const float* v16, const float* e_w
 // ------------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(AGG_WARPS * 32)
 aggregate_h_logits_kernel(const float* __restrict__ logits, const float* __restrict__ vbuf, const float* __restrict__ e_w,
-                          const int* __restrict__ src, const float* __restrict__ h_in, float* __restrict__ h_out, int n_nodes, int k,
+                          const int* __restrict__ src, const float* __restrict__ h_in, float* __restrict__ h_out, TdRows dst, int k,
                           const float* __restrict__ ewm_w, float ewm_b) {
   const int lane = threadIdx.x & 31;
-  const int n = blockIdx.x * AGG_WARPS + (threadIdx.x >> 5);
-  if (n >= n_nodes) return;
+  const long long a = (long long)blockIdx.x * AGG_WARPS + (threadIdx.x >> 5);
+  if (a >= (dst.d_n ? (long long)*dst.d_n : dst.n)) return;
+  const int n = dst.list ? dst.list[a] : (int)a;
+  if (n < 0) return;
   const size_t e0 = (size_t)n * k;
   int deg = 0;
   for (int j = lane; j < k; j += 32) deg += (src[e0 + j] >= 0);
@@ -217,10 +219,10 @@ aggregate_h_logits_kernel(const float* __restrict__ logits, const float* __restr
 }
 
 void td_launch_aggregate_h_logits(const float* logits, const float* vbuf, const float* e_w, const int* src, const float* h_in, float* h_out,
-                                  int n_nodes, int k, const float* ewm_w, float ewm_b, cudaStream_t st) {
-  if (n_nodes == 0) return;
-  aggregate_h_logits_kernel<<<(n_nodes + AGG_WARPS - 1) / AGG_WARPS, AGG_WARPS * 32, 0, st>>>(logits, vbuf, e_w, src, h_in, h_out, n_nodes, k,
-                                                                                             ewm_w, ewm_b);
+                                  const TdRows& dst, int k, const float* ewm_w, float ewm_b, cudaStream_t st) {
+  if (dst.n == 0) return;
+  aggregate_h_logits_kernel<<<(unsigned)((dst.n + AGG_WARPS - 1) / AGG_WARPS), AGG_WARPS * 32, 0, st>>>(logits, vbuf, e_w, src, h_in, h_out, dst, k,
+                                                                                                       ewm_w, ewm_b);
 }
 
 __global__ void __launch_bounds__(AGG_WARPS * 32)

@@ -221,14 +221,18 @@ void td_launch_rel_compact(const unsigned char* flag, int n_nodes, int* rel_list
   rel_compact_kernel<<<(n_nodes + 255) / 256, 256, 0, st>>>(flag, n_nodes, rel_list, n_rel);
 }
 
-// Class-sorted list of the relevant destinations for the v4 edge kernel (last x2h of a sampling step): the relevant PROTEIN nodes,
-// padded with -1 to a multiple of `pad`, followed by the (already padded) list of all ligand nodes.  rel_counts = {entries, protein part}.
+// Class-sorted list of the dirty destinations of one x2h evaluation for the v4 edge kernel (ligand-free cache): the flagged PROTEIN nodes,
+// padded with -1 to a multiple of `pad`, followed by the (already padded) list of all ligand nodes.  counts = {entries, protein part}.
 __global__ void rel_rows_protein_kernel(const unsigned char* __restrict__ flag, const float4* __restrict__ xm, int n_nodes, int* __restrict__ rel_rows,
                                         int* __restrict__ rel_counts) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n_nodes && flag[i] && xm[i].w == 0.0f) rel_rows[atomicAdd(&rel_counts[2], 1)] = i;
 }
-__global__ void rel_rows_finish_kernel(const int* __restrict__ lig_rows, int n_lig_rows, int pad, int* __restrict__ rel_rows, int* __restrict__ rel_counts) {
+// list blockIdx.y (at rows + y * stride, counts + 4 y): its protein part (counts[2] entries) is written; pad it and append the ligand list
+__global__ void rel_rows_finish_kernel(const int* __restrict__ lig_rows, int n_lig_rows, int pad, int* __restrict__ rows, long long stride,
+                                       int* __restrict__ counts) {
+  int* rel_rows = rows + (size_t)blockIdx.y * stride;
+  int* rel_counts = counts + 4 * blockIdx.y;
   const int n_p = rel_counts[2], n_pp = (n_p + pad - 1) / pad * pad;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n_pp - n_p) rel_rows[n_p + i] = -1;
@@ -240,7 +244,93 @@ void td_launch_rel_rows(const unsigned char* rel_flag, const float4* xm, int n_n
   cudaMemsetAsync(rel_counts, 0, 4 * sizeof(int), st);
   if (n_nodes > 0) rel_rows_protein_kernel<<<(n_nodes + 255) / 256, 256, 0, st>>>(rel_flag, xm, n_nodes, rel_rows, rel_counts);
   const int n = n_lig_rows > pad ? n_lig_rows : pad;
-  rel_rows_finish_kernel<<<(n + 255) / 256, 256, 0, st>>>(lig_rows, n_lig_rows, pad, rel_rows, rel_counts);
+  rel_rows_finish_kernel<<<(n + 255) / 256, 256, 0, st>>>(lig_rows, n_lig_rows, pad, rel_rows, 0, rel_counts);
+}
+
+// ---- backward cone of the sampling loop's last block (engine.cu).  A sampling step reads only the ligand rows of the network's output
+// (type head) and the h2x sub-layers read h only on the relevant nodes R (ligand atoms and their neighbours).  x2h evaluation g of the
+// block (G in all) reads h at its destinations and their sources, so it only needs the destinations
+//   R_g = nodes within G - 1 - g hops of R, hops taken from a destination to its sources (R_{G-1} = R, R_{g-1} = R_g + src(R_g)),
+// and its node GEMMs need the A blocks and q on R_g and the B blocks on R_{g-1}.  Rows outside these sets keep stale values.
+// cone_lists_kernel, one CTA per graph (a graph's edges stay inside it): every node's hop distance from R in shared memory, then the
+// protein nodes of 2 G lists, list t at rows + t * stride, its protein count in counts[4 t + 2]:
+//   list 2 g      the destinations R_g of evaluation g (A blocks, q, edge MLPs), of those only the dirty ones for the first `n_dirty`
+//                 (cached) evaluations;
+//   list 2 g + 1  the nodes R_{g-1} (B blocks).
+// rel_rows_finish_kernel then makes each a class-sorted list (every ligand atom is in every R_g and always dirty).  A graph's rows
+// lie in the same order in both lists, so where R_g = R_{g-1} the two column groups of node_proj_kernel read the same h rows at about
+// the same time.  Shared memory: the graph's distances (max_ng ints), then per list a counter and a base (4 G ints).
+#define CONE_THREADS 512
+__global__ void __launch_bounds__(CONE_THREADS)
+cone_lists_kernel(const unsigned char* __restrict__ rel_flag, const int* __restrict__ src, const int* __restrict__ node_ptr,
+                  const float4* __restrict__ xm, int n_nodes, int k, int G, int max_ng, const unsigned char* __restrict__ dirty, int n_dirty,
+                  int* __restrict__ rows, long long stride, int* __restrict__ counts) {
+  extern __shared__ int s_dist[];
+  int* s_cnt = s_dist + max_ng;                  // [2 G]
+  int* s_base = s_cnt + 2 * G;
+  const int n0 = node_ptr[blockIdx.x], ng = node_ptr[blockIdx.x + 1] - n0;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  constexpr int kFar = 1 << 30;
+  for (int i = threadIdx.x; i < ng; i += blockDim.x) s_dist[i] = rel_flag[n0 + i] ? 0 : kFar;
+  for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) s_cnt[i] = 0;
+  __syncthreads();
+  // breadth-first rounds: round r gives the unvisited sources of the nodes at distance r distance r + 1.  Round r only writes r + 1, so a
+  // node's `== r` test is stable (and warp-uniform) while other warps write.
+  for (int r = 0; r < G; ++r) {
+    bool grew = false;
+    for (int i = warp; i < ng; i += nw) {
+      if (s_dist[i] != r) continue;
+      for (int j = lane; j < k; j += 32) {
+        const int s = src[(size_t)(n0 + i) * k + j];
+        if (s >= 0 && s_dist[s - n0] > r + 1) { s_dist[s - n0] = r + 1; grew = true; }
+      }
+    }
+    if (!__syncthreads_or(grew)) break;
+  }
+  // two passes over the graph's nodes, 32 per warp: count every list's members, reserve the graph's ranges, write
+  const unsigned lt = (1u << lane) - 1u;
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int i0 = 32 * warp; i0 < ng; i0 += 32 * nw) {
+      const int i = i0 + lane, n = n0 + i;
+      const int d = i < ng ? s_dist[i] : kFar;
+      const bool prot = i < ng && xm[n].w == 0.0f;
+      for (int g = 0; g < G; ++g) {
+        const bool a = prot && d <= G - 1 - g && (g >= n_dirty || dirty[(size_t)g * n_nodes + n]);
+        const bool b = prot && d <= G - g;
+        const unsigned ma = __ballot_sync(0xffffffffu, a), mb = __ballot_sync(0xffffffffu, b);
+        int oa = 0, ob = 0;
+        if (lane == 0) {
+          if (ma) oa = atomicAdd(&s_cnt[2 * g], __popc(ma));
+          if (mb) ob = atomicAdd(&s_cnt[2 * g + 1], __popc(mb));
+        }
+        if (pass == 0) continue;
+        oa = __shfl_sync(0xffffffffu, oa, 0);
+        ob = __shfl_sync(0xffffffffu, ob, 0);
+        if (a) rows[(size_t)(2 * g) * stride + s_base[2 * g] + oa + __popc(ma & lt)] = n;
+        if (b) rows[(size_t)(2 * g + 1) * stride + s_base[2 * g + 1] + ob + __popc(mb & lt)] = n;
+      }
+    }
+    __syncthreads();
+    if (pass == 0) {
+      for (int t = threadIdx.x; t < 2 * G; t += blockDim.x) {
+        s_base[t] = s_cnt[t] ? atomicAdd(&counts[4 * t + 2], s_cnt[t]) : 0;
+        s_cnt[t] = 0;
+      }
+      __syncthreads();
+    }
+  }
+}
+void td_launch_cone_lists(const unsigned char* rel_flag, const int* src, const int* node_ptr, const float4* xm, int n_graphs, int max_ng, int n_nodes,
+                          int k, int G, const unsigned char* dirty, int n_dirty, const int* lig_rows, int n_lig_rows, int pad, int* rows,
+                          long long stride, int* counts, cudaStream_t st) {
+  if (G <= 0) return;
+  cudaMemsetAsync(counts, 0, (size_t)G * 8 * sizeof(int), st);
+  const size_t smem = ((size_t)max_ng + 4 * (size_t)G) * sizeof(int);
+  static size_t opted[TD_MAX_DEVICES] = {0};
+  td_opt_in_smem(cone_lists_kernel, smem, opted);
+  cone_lists_kernel<<<n_graphs, CONE_THREADS, smem, st>>>(rel_flag, src, node_ptr, xm, n_nodes, k, G, max_ng, dirty, n_dirty, rows, stride, counts);
+  const int n = n_lig_rows > pad ? n_lig_rows : pad;
+  rel_rows_finish_kernel<<<dim3((n + 255) / 256, 2 * G), 256, 0, st>>>(lig_rows, n_lig_rows, pad, rows, stride, counts);
 }
 
 // ---- ligand-free cache support (engine.cu): a node's features after x2h layer l equal their ligand-free values unless the node is

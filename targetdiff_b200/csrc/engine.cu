@@ -98,7 +98,7 @@ struct tdiff_engine {
               *t_sra = nullptr, *t_srm1 = nullptr, *t_ac = nullptr;
   // ---- batch
   bool bound = false, has_ligand = false, have_graph = false;
-  bool restrict_last = false;           // sampling loop only: the last layer's x2h is evaluated for the relevant nodes only
+  bool restrict_last = false;           // sampling loop only: the last block's x2h evaluations run on the backward cone of the ligand (cone_rows)
   bool knn_incremental = false;         // protein-protein neighbour keys cached at bind time (TDIFF_KNN_FULL=1 disables)
   bool have_prev = false;               // src_prev / etype / e_w hold the previous forward's graph of this batch (edge_const reuse)
   // developer switches, read from the environment ONCE in tdiff_create (never on the per-layer path)
@@ -110,8 +110,13 @@ struct tdiff_engine {
   DevBuf node_ptr, prot_ptr, prot_node, prot_graph, lig_node, lig_graph, node_lig;
   DevBuf rel_flag, rel_list, n_rel, work_list, n_work, knn_cache;
   // class-sorted destination lists of the v4 edge kernel: protein destinations (padded with -1 to `row_pad`), then ligand destinations
-  DevBuf x2h_rows, lig_rows, rel_rows, rel_counts;
+  DevBuf x2h_rows, lig_rows;
   long long x2h_n_dst = 0, x2h_split = 0, lig_n_dst = 0;
+  // backward cone of the sampling loop's last block (edge_const.cu, cone_lists_kernel), per x2h evaluation g two class-sorted lists
+  // (stride free_stride): cone_rows[2 g] the destinations R_g, cone_rows[2 g + 1] the nodes R_{g-1}; cone_counts[4 t ..] = {entries,
+  // protein part, protein nodes, -} of list t
+  DevBuf cone_rows, cone_counts;
+  int cone_evals = 0;                   // evaluations the cone lists hold (0: not built since the batch was bound)
   int row_pad = 4;                      // destinations per class are padded so that class boundaries fall on 128-row tile boundaries
   // Ligand-free cache (exact): protein atoms never move and their embedding is step-invariant, so a protein node that is neither
   // touched by a ligand atom nor (transitively, x2h evaluation by evaluation) fed by a touched node has the same features after x2h
@@ -627,7 +632,7 @@ extern "C" void tdiff_destroy(tdiff_engine* e) {
   if (e->ev_fork) cudaEventDestroy(e->ev_fork);
   if (e->ev_join) cudaEventDestroy(e->ev_join);
   DevBuf* bufs[] = {&e->node_ptr, &e->prot_ptr, &e->prot_node, &e->prot_graph, &e->lig_node, &e->lig_graph, &e->node_lig, &e->xm0, &e->xm1,
-                    &e->rel_flag, &e->rel_list, &e->n_rel, &e->work_list, &e->n_work, &e->knn_cache, &e->x2h_rows, &e->lig_rows, &e->rel_rows, &e->rel_counts, &e->ew_x2h, &e->ew_h2x, &e->h_sync, &e->hagg, &e->time_norm, &e->h_free, &e->dirty, &e->free_rows, &e->free_counts, &e->lig_save, &e->offset, &e->h0, &e->h, &e->P, &e->q, &e->src, &e->src_prev, &e->etype, &e->e_w, &e->dist, &e->kbuf, &e->vbuf, &e->v16, &e->lig_pos,
+                    &e->rel_flag, &e->rel_list, &e->n_rel, &e->work_list, &e->n_work, &e->knn_cache, &e->x2h_rows, &e->lig_rows, &e->cone_rows, &e->cone_counts, &e->ew_x2h, &e->ew_h2x, &e->h_sync, &e->hagg, &e->time_norm, &e->h_free, &e->dirty, &e->free_rows, &e->free_counts, &e->lig_save, &e->offset, &e->h0, &e->h, &e->P, &e->q, &e->src, &e->src_prev, &e->etype, &e->e_w, &e->dist, &e->kbuf, &e->vbuf, &e->v16, &e->lig_pos,
                     &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges, &e->fix_mask, &e->fix_pos, &e->fix_v, &e->seq_buf, &e->lk_buf, &e->lk_x0, &e->lk_v0};
   for (auto* b : bufs) b->release();
   for (auto& b : e->stage) b.release();
@@ -680,7 +685,7 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
     for (int i = 0; i < lc[g]; ++i) { lig_node[a] = n; lig_graph[a] = g; node_lig[n] = a; ++a; ++n; }
   }
   node_ptr[B] = n; prot_ptr[B] = p;
-  e->bound = false; e->has_ligand = false; e->have_graph = false; e->have_prev = false;
+  e->bound = false; e->has_ligand = false; e->have_graph = false; e->have_prev = false; e->cone_evals = 0;
   e->has_fixed = false; e->fix_pos_noise = nullptr; e->fix_v_uniform = nullptr;
   e->start_t = -1; e->start_pos_noise = nullptr; e->start_v_uniform = nullptr;
   e->B = B; e->N = (int)N; e->Np = (int)Np; e->Nl = (int)Nl; e->max_ng = max_ng;
@@ -701,8 +706,9 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   std::vector<int> x2h_rows((size_t)(nPpad + nLpad), -1), lig_rows((size_t)nLpad, -1);
   for (long long i = 0; i < Np; ++i) x2h_rows[i] = prot_node[i];
   for (long long i = 0; i < Nl; ++i) { x2h_rows[nPpad + i] = lig_node[i]; lig_rows[i] = lig_node[i]; }
-  if (v4) bad |= e->x2h_rows.ensure(x2h_rows.size() * 4 + 4) | e->lig_rows.ensure(lig_rows.size() * 4 + 4) | e->rel_rows.ensure(x2h_rows.size() * 4 + 4) |
-                 e->rel_counts.ensure(16);
+  const size_t x2h_evals = e->layers.size() * (size_t)e->num_x2h;
+  if (v4) bad |= e->x2h_rows.ensure(x2h_rows.size() * 4 + 4) | e->lig_rows.ensure(lig_rows.size() * 4 + 4) |
+                 e->cone_rows.ensure(2 * x2h_evals * x2h_rows.size() * 4 + 4) | e->cone_counts.ensure(2 * x2h_evals * 16 + 16);
   // per-edge buffers: v4 keeps 16 attention logits / weights per row and, with the aggregation fused into the value launch (k == 32),
   // no [E,128] tensor at all; the earlier execution modes materialise keys and values
   const bool fuse = v4 && K == 32 && !e->env_no_fused_agg && e->ew_mode != 2;      // 'm' gates need the value rows (unfused aggregation)
@@ -719,9 +725,8 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   for (int g = 0; g < B; ++g) if (pc[g] < min_pc) min_pc = pc[g];
   e->free_ready = false;
   e->free_depth = (fuse && !e->hybrid && Nl > 0 && min_pc > K) ? e->env_free_depth : 0;      // (only block 0 of a multi-block network uses it)
-  // counted in x2h sub-layer evaluations of block 0; the last one may be restricted to the relevant nodes and is never cached
-  const int x2h_evals = (int)e->layers.size() * e->num_x2h;
-  if (e->free_depth > x2h_evals - 1) e->free_depth = x2h_evals - 1 > 0 ? x2h_evals - 1 : 0;
+  // counted in x2h sub-layer evaluations of block 0; the last one is never cached
+  if (e->free_depth > (int)x2h_evals - 1) e->free_depth = (int)x2h_evals - 1 > 0 ? (int)x2h_evals - 1 : 0;
   if (e->free_depth > 0)
     bad |= e->h_free.ensure((size_t)e->free_depth * N * TD_H * 4) | e->dirty.ensure((size_t)e->free_depth * N + 16) |
            e->free_rows.ensure((size_t)e->free_depth * x2h_rows.size() * 4 + 4) | e->free_counts.ensure((size_t)e->free_depth * 16) |
@@ -869,27 +874,27 @@ struct Prof {
   ~Prof() { if (on) { cudaEventRecord(ev.b, st); e->events.push_back(ev); } }
 };
 
-// per-edge MLP dispatch.  `list`: which destination set the launch covers.
+// per-edge MLP dispatch.  `list`: which destination set the launch covers; `sub` (v4 only): a device-counted subset of the ROWS_ALL list
+// in the same class-sorted layout (the dirty destinations of a cached evaluation, or the backward cone of the sampling loop).
 //   v4 (default): class-sorted destination lists; `qnode` != NULL marks a key MLP whose output is 16 attention logits (or, with
 //   `key_softmax`, softmax weights * e_w) per row; `agg_logits` / `agg_h` make the value launch perform the attention aggregation.
 //   earlier modes: tensor-core second Linear with keys / values in HBM (edge_mlp_tc.cu) or the FP32 FFMA build (edge_mlp.cu).
-enum RowList { ROWS_ALL = 0, ROWS_LIGAND = 1, ROWS_RELEVANT = 2 };
+enum RowList { ROWS_ALL = 0, ROWS_LIGAND = 1 };
+struct SubRows {
+  const int* rows = nullptr;       // class-sorted destination list
+  const int* counts = nullptr;     // device {entries, protein part}
+};
 bool fused_logits(const tdiff_engine* e) { return e->mlp_mode == 2 && e->mlp_v4; }
 void edge_mlp(tdiff_engine* e, const float* P, const float4* xm, const int* src, const unsigned char* etype, RowList list, int K, const TdMlp& m,
               const float* offsets, float coeff, float* out, cudaStream_t st, const float* e_w, const float* qnode = nullptr,
-              const float* agg_logits = nullptr, float* agg_h = nullptr, int key_softmax = 0, int free_layer = -1) {
+              const float* agg_logits = nullptr, float* agg_h = nullptr, int key_softmax = 0, SubRows sub = SubRows()) {
   if (fused_logits(e) && m.w2_img && m.tabcls_img) {
-    const int* rows = list == ROWS_ALL ? e->x2h_rows.as<int>() : list == ROWS_LIGAND ? e->lig_rows.as<int>() : e->rel_rows.as<int>();
-    const int* counts = list == ROWS_RELEVANT ? e->rel_counts.as<int>() : nullptr;
-    if (free_layer >= 0) {           // ligand-free cache: only the dirty destinations of this layer (device-compacted, class-sorted)
-      rows = e->free_rows.as<int>() + (size_t)free_layer * e->free_stride;
-      counts = e->free_counts.as<int>() + 4 * free_layer;
-    }
-    const long long n_dst = list == ROWS_LIGAND ? e->lig_n_dst : e->x2h_n_dst;          // ROWS_RELEVANT: upper bound, real counts on the device
+    const int* rows = sub.rows ? sub.rows : list == ROWS_ALL ? e->x2h_rows.as<int>() : e->lig_rows.as<int>();
+    const long long n_dst = list == ROWS_LIGAND ? e->lig_n_dst : e->x2h_n_dst;          // with `sub`: upper bound, real counts on the device
     const long long split = list == ROWS_LIGAND ? 0 : e->x2h_split;
     // plain (unfused) x2h outputs are consumed by slot index (aggregate_h_logits_kernel); everything else by row index
     const int by_slot = (list != ROWS_LIGAND && !key_softmax && agg_logits == nullptr) ? 1 : 0;
-    td_launch_edge_mlp_v4(P, e->N, src, etype, e->dist.as<float>(), rows, n_dst, split, counts, K, m,
+    td_launch_edge_mlp_v4(P, e->N, src, etype, e->dist.as<float>(), rows, n_dst, split, sub.counts, K, m,
                           e->host_arena.data() + (offsets - e->arena), coeff, e->host_arena.data() + (m.ln_b - e->arena),
                           e->host_arena.data() + (m.b2 - e->arena), qnode, out, by_slot, agg_logits, e_w, agg_h, key_softmax,
                           e->sm_count, st);
@@ -904,18 +909,19 @@ void edge_mlp(tdiff_engine* e, const float* P, const float4* xm, const int* src,
 }
 
 // node-side GEMMs: P = h . Wn^T + bn ; q = relu(LN(P[:,512:640])) . W2q^T + b2q   (tensor cores unless TDIFF_EDGE_MLP=simt)
-// `rows` / `d_n` (optional): restrict to a node subset given as a device list (+ device count); other rows of P / q are left stale
 // Default mode (v4 edge MLPs): node_side.cu computes P[:, 0:512] and q from h, q_pre stays in registers (P[:, 512:640] is not written:
-// the v4 edge MLPs do not read it).
-void node_side(tdiff_engine* e, const float* h, int N, const TdSubLayer& sl, float* P, float* q, cudaStream_t st, const int* rows = nullptr,
-               const int* d_n = nullptr) {
+// the v4 edge MLPs do not read it); `rows_a` / `rows_b` (optional, v4 only): node subsets for the A blocks and q (read at edge
+// destinations) and for the B blocks (read at edge sources); other rows of P / q are left stale.
+void node_side(tdiff_engine* e, const float* h, int N, const TdSubLayer& sl, float* P, float* q, cudaStream_t st, const TdRows* rows_a = nullptr,
+               const TdRows* rows_b = nullptr) {
   if (fused_logits(e) && sl.wn_img && sl.q.w2_img) {
-    td_launch_node_side_v4(h, N, sl.wn_img, sl.bn, sl.q, P, q, rows, d_n, e->sm_count, st);
+    const TdRows all = {nullptr, nullptr, N};
+    td_launch_node_side_v4(h, sl.wn_img, sl.bn, sl.q, P, q, rows_a ? *rows_a : all, rows_b ? *rows_b : all, e->sm_count, st);
   } else if (e->mlp_mode != 0 && sl.wn_img && sl.q.w2_img) {
     TdMlp pm = sl.q;
     pm.b2 = sl.bn;                 // mode 1 reads the per-column-block bias through m.b2
-    td_launch_rows_tc(1, h, TD_H, 0, N, pm, sl.wn_img, e->mlp_mode, P, TD_NPROJ, TD_NPROJ / TD_H, rows, d_n, e->sm_count, st);
-    td_launch_rows_tc(2, P, TD_NPROJ, 512, N, sl.q, sl.q.w2_img, e->mlp_mode, q, TD_H, 1, rows, d_n, e->sm_count, st);
+    td_launch_rows_tc(1, h, TD_H, 0, N, pm, sl.wn_img, e->mlp_mode, P, TD_NPROJ, TD_NPROJ / TD_H, nullptr, nullptr, e->sm_count, st);
+    td_launch_rows_tc(2, P, TD_NPROJ, 512, N, sl.q, sl.q.w2_img, e->mlp_mode, q, TD_H, 1, nullptr, nullptr, e->sm_count, st);
   } else {
     td_launch_node_proj(h, N, sl.wn_t, sl.bn, P, st);
     td_launch_node_q(P, N, sl.q, q, st);
@@ -974,14 +980,21 @@ void run_forward(tdiff_engine* e, cudaStream_t st, int fix_x, int free_build = 0
     }
     td_launch_rel_compact(e->rel_flag.as<unsigned char>(), N, e->rel_list.as<int>(), e->n_rel.as<int>(), st);
     e->launches += 4;
-    if (fused_logits(e) && e->restrict_last && last_blk && e->num_x2h > 0) {   // class-sorted list of the relevant destinations for the last x2h
-      td_launch_rel_rows(e->rel_flag.as<unsigned char>(), xm[cur], N, e->lig_rows.as<int>(), (int)e->lig_n_dst, e->row_pad, e->rel_rows.as<int>(),
-                         e->rel_counts.as<int>(), st);
-      e->launches += 2;
-    }
     const float4* xm_blk = xm[cur];                  // coordinates the block's graph was built from (protein flags for the cache kernels)
     const int NX = e->num_x2h, NH = e->num_h2x;
     const size_t L = e->layers.size();
+    // sampling loop, last block: only the ligand rows of h feed the type head and only the relevant nodes (ligand atoms and their
+    // neighbours) feed the h2x sub-layers, so every x2h evaluation runs on the backward cone of those rows (edge_const.cu,
+    // cone_lists_kernel; h of other rows, final_h included, is left stale).  node_output (x2h_out_fc) reads every row of h.
+    const bool cone = fused_logits(e) && e->restrict_last && last_blk && NX > 0 && !e->env_no_restrict && !e->out_fc;
+    const long long cone_stride = e->free_stride;
+    if (cone) {
+      td_launch_cone_lists(e->rel_flag.as<unsigned char>(), src, e->node_ptr.as<int>(), xm_blk, e->B, e->max_ng, N, K, (int)L * NX,
+                           use_free ? e->dirty.as<unsigned char>() : nullptr, use_free, e->lig_rows.as<int>(), (int)e->lig_n_dst, e->row_pad,
+                           e->cone_rows.as<int>(), cone_stride, e->cone_counts.as<int>(), st);
+      e->launches += 2;
+      e->cone_evals = (int)L * NX;
+    }
     int g = 0;                                       // x2h sub-layer evaluations of this block so far (the ligand-free cache's unit)
     for (size_t l = 0; l < L && !(free_build && g >= free_build); ++l) {
       const TdLayer& ly = e->layers[l];
@@ -999,8 +1012,20 @@ void run_forward(tdiff_engine* e, cudaStream_t st, int fix_x, int free_build = 0
       for (int i = 0; i < NX && !(free_build && g >= free_build); ++i, ++g) {
         const TdSubLayer& sx = ly.x2h[i];
         const int fl = g < use_free ? g : -1;
+        // destinations of this evaluation: the cone (dirty ones only on cached evaluations), the dirty ones, or all
+        SubRows sub;
+        TdRows rows_a = {nullptr, nullptr, N}, rows_b = {nullptr, nullptr, N};
+        if (cone) {
+          sub.rows = e->cone_rows.as<int>() + (size_t)(2 * g) * cone_stride;
+          sub.counts = e->cone_counts.as<int>() + 8 * g;
+          rows_a = {sub.rows, sub.counts, e->x2h_n_dst};
+          rows_b = {sub.rows + cone_stride, sub.counts + 4, e->x2h_n_dst};
+        } else if (fl >= 0) {
+          sub.rows = e->free_rows.as<int>() + (size_t)fl * e->free_stride;
+          sub.counts = e->free_counts.as<int>() + 4 * fl;
+        }
         // ---- x2h: h <- h + sum_e alpha * v * e_w   (+ node_output MLP with x2h_out_fc)
-        node_side(e, h, N, sx, P, q, st);
+        node_side(e, h, N, sx, P, q, st, &rows_a, &rows_b);
         // edge lengths from the layer's input coordinates (x does not move during x2h); 'r': this x2h sub-layer's gates and the first
         // h2x sub-layer's (with no h2x sub-layer, a throw-away second set)
         if (e->mlp_mode != 0 && (i == 0 || e->ew_mode == 1)) {
@@ -1014,11 +1039,6 @@ void run_forward(tdiff_engine* e, cudaStream_t st, int fix_x, int free_build = 0
         }
         // k == 32: a 128-row tile is 4 complete destinations -> the value launch also performs the softmax aggregation (h += ...)
         const bool fuse_agg = fused_logits(e) && K == 32 && !e->env_no_fused_agg && e->ew_mode != 2;
-        // sampling loop, last x2h sub-layer of the network: only the ligand atoms' features feed the type head and only ligand atoms +
-        // their neighbours feed the h2x sub-layers, so x2h is evaluated for those destinations only (device-compacted list; final_h of
-        // other nodes is not produced).  With sync_twoup the h2x sub-layers read the layer's input h, and the head the ligand rows.
-        const bool sub = fuse_agg && e->restrict_last && last_blk && l + 1 == L && i + 1 == NX && !e->env_no_restrict && !e->out_fc;
-        const RowList rl = sub ? ROWS_RELEVANT : ROWS_ALL;
         float* agg_target = h;
         if (e->out_fc) {               // node_output needs the bare aggregate: accumulate into a zeroed buffer instead of h
           agg_target = e->hagg.as<float>();
@@ -1026,16 +1046,16 @@ void run_forward(tdiff_engine* e, cudaStream_t st, int fix_x, int free_build = 0
         }
         {
           Prof pr(e, st, EV_EDGE_MLP);
-          edge_mlp(e, P, xm[cur], src, etype, rl, K, sx.k, ly.offsets, ly.coeff, e->kbuf.as<float>(), st, ew_x, fused_logits(e) ? q : nullptr, nullptr,
-                   nullptr, fuse_agg ? 1 : 0, fl);
-          edge_mlp(e, P, xm[cur], src, etype, rl, K, sx.v, ly.offsets, ly.coeff, e->vbuf.as<float>(), st, ew_x, nullptr,
-                   fuse_agg ? e->kbuf.as<float>() : nullptr, fuse_agg ? agg_target : nullptr, 0, fl);
+          edge_mlp(e, P, xm[cur], src, etype, ROWS_ALL, K, sx.k, ly.offsets, ly.coeff, e->kbuf.as<float>(), st, ew_x, fused_logits(e) ? q : nullptr,
+                   nullptr, nullptr, fuse_agg ? 1 : 0, sub);
+          edge_mlp(e, P, xm[cur], src, etype, ROWS_ALL, K, sx.v, ly.offsets, ly.coeff, e->vbuf.as<float>(), st, ew_x, nullptr,
+                   fuse_agg ? e->kbuf.as<float>() : nullptr, fuse_agg ? agg_target : nullptr, 0, sub);
         }
         if (!fuse_agg) {
           Prof pr(e, st, EV_AGG_H);
           if (fused_logits(e))
-            td_launch_aggregate_h_logits(e->kbuf.as<float>(), e->vbuf.as<float>(), ew_x, src, e->out_fc ? agg_target : h, agg_target, N, K,
-                                         e->ew_mode == 2 ? sx.ew_w : nullptr, sx.ew_b, st);
+            td_launch_aggregate_h_logits(e->kbuf.as<float>(), e->vbuf.as<float>(), ew_x, src, e->out_fc ? agg_target : h, agg_target,
+                                         sub.rows ? rows_a : TdRows{nullptr, nullptr, N}, K, e->ew_mode == 2 ? sx.ew_w : nullptr, sx.ew_b, st);
           else td_launch_aggregate_h(e->kbuf.as<float>(), e->vbuf.as<float>(), e->e_w.as<float>(), src, q, h, h, N, K, st);
         }
         e->launches += fuse_agg ? 4 : 5;
@@ -1068,9 +1088,11 @@ void run_forward(tdiff_engine* e, cudaStream_t st, int fix_x, int free_build = 0
                                    ly.offsets, ly.coeff, e->ew_h2x.as<float>(), st);
           e->launches += 1;
         }
-        {
-          const bool rel = fused_logits(e) && !e->env_no_restrict;      // h2x only reads P / q of ligand atoms and their neighbours
-          node_side(e, h_h2x, N, sh, P, q, st, rel ? e->rel_list.as<int>() : nullptr, rel ? e->n_rel.as<int>() : nullptr);
+        if (fused_logits(e) && !e->env_no_restrict) {   // h2x reads the A blocks and q at the ligand atoms, the B blocks at their neighbours
+          const TdRows rows_a = {e->lig_node.as<int>(), nullptr, Nl}, rows_b = {e->rel_list.as<int>(), e->n_rel.as<int>(), N};
+          node_side(e, h_h2x, N, sh, P, q, st, &rows_a, &rows_b);
+        } else {
+          node_side(e, h_h2x, N, sh, P, q, st);
         }
         {
           Prof pr(e, st, EV_EDGE_MLP);
@@ -1600,6 +1622,17 @@ extern "C" int tdiff_check_stability(const float* d_pos, const int32_t* d_atomic
 
 // ---------------------------------------------------------------------------------------------- instrumentation
 extern "C" int64_t tdiff_launch_count(tdiff_engine* e) { return e ? e->launches : 0; }
+
+extern "C" int tdiff_get_cone(tdiff_engine* e, int32_t* h_dims, int32_t* h_counts, int32_t* h_rows) {
+  if (!e || !h_dims) return set_err(TDIFF_EINVAL, "get_cone: bad arguments");
+  if (!e->bound || e->cone_evals == 0) return set_err(TDIFF_ESTATE, "get_cone: no sampling step has built the cone lists of this batch");
+  CK(cudaSetDevice(e->device));
+  const size_t G = (size_t)e->cone_evals, stride = (size_t)e->free_stride;
+  h_dims[0] = (int32_t)G; h_dims[1] = (int32_t)stride;
+  if (h_counts) CK(cudaMemcpy(h_counts, e->cone_counts.p, 2 * G * 16, cudaMemcpyDeviceToHost));
+  if (h_rows) CK(cudaMemcpy(h_rows, e->cone_rows.p, 2 * G * stride * 4, cudaMemcpyDeviceToHost));
+  return TDIFF_OK;
+}
 extern "C" int tdiff_edge_mlp_mode(tdiff_engine* e) { return !e ? TDIFF_EINVAL : (e->mlp_mode == 2 && e->mlp_v4) ? 5 : e->mlp_mode; }
 
 extern "C" int tdiff_profile(tdiff_engine* e, int enable) {

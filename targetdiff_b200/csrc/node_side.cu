@@ -60,26 +60,27 @@ __device__ __forceinline__ void stage_weights(unsigned char* sW, const unsigned 
   __syncthreads();
 }
 
-struct Rows {
-  const int* list;       // optional: logical row i is node list[i]
-  const int* d_n;        // optional: number of logical rows, in device memory
-  long long n;           // number of logical rows (upper bound with d_n)
-};
+using Rows = TdRows;
 
 // A warpgroup's h tile in shared memory: 64 rows of 512 B, 16-byte chunk c of row r at chunk position c ^ 2 (r % 4), which makes both
 // the row-wise copies and the fragment-order reads below free of bank conflicts.
 __device__ __forceinline__ uint32_t chunk_pos(int r, int c) { return (uint32_t)(r * 512 + ((c ^ ((r & 3) << 1)) << 4)); }
 __device__ __forceinline__ void bar_sync_wg(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-// cp.async of tile `tile`'s 64 h rows into the buffer at `buf` (rows past the end are zero-filled); warp w copies rows w, w + 4, ...
+// cp.async of tile `tile`'s 64 h rows into the buffer at `buf` (rows past the end and padding entries are zero-filled); warp w copies rows w, w + 4, ...
+// The list entries of the warp's 16 rows are loaded once, one per lane, so that the copies are not issued behind 16 dependent loads.
 __device__ __forceinline__ void load_tile_async(uint32_t buf, const float* __restrict__ in, const Rows& rw, long long n, long long tile, int t) {
   const int l = t & 31;
+  long long mine = -1;
+  if (l < kTile / 4) {
+    const long long i = tile * kTile + (t >> 5) + 4 * l;
+    mine = i < n ? (rw.list ? (long long)rw.list[i] : i) : -1;
+  }
 #pragma unroll 1
-  for (int r = t >> 5; r < kTile; r += 4) {
-    const long long i = tile * kTile + r;
-    const long long node = i < n ? (rw.list ? (long long)rw.list[i] : i) : 0;
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(buf + chunk_pos(r, l)), "l"(in + (size_t)node * TD_H + 4 * l),
-                 "r"(i < n ? 16 : 0) : "memory");
+  for (int r = t >> 5, j = 0; r < kTile; r += 4, ++j) {
+    const long long node = __shfl_sync(0xffffffffu, mine, j);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(buf + chunk_pos(r, l)), "l"(in + (size_t)(node >= 0 ? node : 0) * TD_H + 4 * l),
+                 "r"(node >= 0 ? 16 : 0) : "memory");
   }
   asm volatile("cp.async.commit_group;" ::: "memory");
 }
@@ -172,11 +173,13 @@ __device__ __forceinline__ void tile_rows(const Rows& rw, long long n, long long
 
 }  // namespace ns
 
-// grid (CTAs per column group, 2): column group g = blockIdx.y writes P columns 256 g .. 256 g + 255 (weight blocks 2 g, 2 g + 1)
+// grid (CTAs per column group, 2): column group g = blockIdx.y writes P columns 256 g .. 256 g + 255 (weight blocks 2 g, 2 g + 1) of the
+// rows of rw[g]: group 0 the A blocks [A_k | A_v] (read at edge destinations), group 1 the B blocks [B_k | B_v] (read at edge sources)
 __global__ void __launch_bounds__(ns::kThreads, 1)
 node_proj_kernel(const float* __restrict__ h, const unsigned char* __restrict__ wn_img, const float* __restrict__ bn, float* __restrict__ P,
-                 ns::Rows rw) {
+                 const ns::Rows rw_a, const ns::Rows rw_b) {
   using namespace ns;
+  const Rows rw = blockIdx.y ? rw_b : rw_a;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* sW = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   float* sBias = reinterpret_cast<float*>(sW + 2 * kBlock + kWG * kHBuf);
@@ -275,20 +278,20 @@ node_query_kernel(const float* __restrict__ h, const unsigned char* __restrict__
   }
 }
 
-// Node-side GEMMs of one sub-layer (2 launches): P[:, 0:512] and q.  `rows` / `d_n` (optional): only the listed nodes (count in device
-// memory; n_rows is then the upper bound that sizes the grids); other rows of P / q are left as they were.
-void td_launch_node_side_v4(const float* h, long long n_rows, const unsigned char* wn_img, const float* bn, const TdMlp& q_mlp, float* P,
-                            float* q, const int* rows, const int* d_n, int sm_count, cudaStream_t st) {
+// Node-side GEMMs of one sub-layer (2 launches): the A blocks of P and q on the rows of `rows_a`, the B blocks of P on the rows of
+// `rows_b`; other rows of P / q are left as they were.  The host bounds `n` size the grids.
+void td_launch_node_side_v4(const float* h, const unsigned char* wn_img, const float* bn, const TdMlp& q_mlp, float* P, float* q, const TdRows& rows_a,
+                            const TdRows& rows_b, int sm_count, cudaStream_t st) {
   using namespace ns;
-  if (n_rows == 0) return;
+  if (rows_a.n == 0 && rows_b.n == 0) return;
   static size_t opted_p[TD_MAX_DEVICES] = {0}, opted_q[TD_MAX_DEVICES] = {0};
   td_opt_in_smem(node_proj_kernel, kSmem, opted_p);
   td_opt_in_smem(node_query_kernel, kSmem, opted_q);
-  const Rows rw = {rows, d_n, n_rows};
-  const long long slots = (n_rows + kTile - 1) / kTile;            // warpgroup tiles
-  const long long ctas = (slots + kWG - 1) / kWG;
+  auto ctas = [](long long n_rows) { return ((n_rows + kTile - 1) / kTile + kWG - 1) / kWG; };     // warpgroup tiles -> CTAs
+  const long long cp = ctas(rows_a.n > rows_b.n ? rows_a.n : rows_b.n), cq = ctas(rows_a.n);
   const int per = sm_count / 2 > 0 ? sm_count / 2 : 1;
-  node_proj_kernel<<<dim3((unsigned)(ctas < per ? ctas : per), 2), kThreads, kSmem, st>>>(h, wn_img, bn, P, rw);
-  node_query_kernel<<<(unsigned)(ctas < sm_count ? ctas : sm_count), kThreads, kSmem, st>>>(h, wn_img + 4 * (size_t)kImgStride, bn + 512, q_mlp,
-                                                                                           q, rw);
+  node_proj_kernel<<<dim3((unsigned)(cp < per ? cp : per), 2), kThreads, kSmem, st>>>(h, wn_img, bn, P, rows_a, rows_b);
+  if (cq > 0)
+    node_query_kernel<<<(unsigned)(cq < sm_count ? cq : sm_count), kThreads, kSmem, st>>>(h, wn_img + 4 * (size_t)kImgStride, bn + 512, q_mlp, q,
+                                                                                         rows_a);
 }

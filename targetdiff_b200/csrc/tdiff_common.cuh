@@ -152,6 +152,9 @@ void td_launch_dirty_propagate(const unsigned char* in, const int* src, int n_no
 void td_launch_restore_clean(const unsigned char* dirty, const float4* xm, const float* h_free, int n_nodes, float* h, cudaStream_t st);
 void td_launch_rel_rows(const unsigned char* rel_flag, const float4* xm, int n_nodes, const int* lig_rows, int n_lig_rows, int pad, int* rel_rows,
                         int* rel_counts, cudaStream_t st);
+void td_launch_cone_lists(const unsigned char* rel_flag, const int* src, const int* node_ptr, const float4* xm, int n_graphs, int max_ng, int n_nodes,
+                          int k, int G, const unsigned char* dirty, int n_dirty, const int* lig_rows, int n_lig_rows, int pad, int* rows,
+                          long long stride, int* counts, cudaStream_t st);
 void td_launch_protein_embed(const float* feat, int n_protein, int fdim, const float* w, const float* b, const int* prot_node,
                              float* h0, cudaStream_t st);
 void td_launch_init_h(const float* h0, const float4* xm, const int* lig_v, const int* node_lig, const float* wl_t, const float* bl,
@@ -175,15 +178,22 @@ void td_launch_edge_mlp_v4(const float* P, int zero_row, const int* src, const u
                            const float* agg_logits, const float* agg_e_w, float* agg_h, int key_softmax, int sm_count, cudaStream_t st);
 void td_launch_rows_tc(int mode, const float* in, int ldi, int in_off, long long n_rows, TdMlp m, const unsigned char* w_image, int pieces, float* out,
                        int ldo, int nblocks, const int* row_list, const int* d_n_rows, int sm_count, cudaStream_t st);
-void td_launch_node_side_v4(const float* h, long long n_rows, const unsigned char* wn_img, const float* bn, const TdMlp& q_mlp, float* P,
-                            float* q, const int* rows, const int* d_n, int sm_count, cudaStream_t st);
+// a node subset: logical row i is node list[i] (entries < 0 are padding and skipped), or i without a list; rows below *d_n, or below n
+// without d_n (n then bounds *d_n from above)
+struct TdRows {
+  const int* list;
+  const int* d_n;
+  long long n;
+};
+void td_launch_node_side_v4(const float* h, const unsigned char* wn_img, const float* bn, const TdMlp& q_mlp, float* P, float* q, const TdRows& rows_a,
+                            const TdRows& rows_b, int sm_count, cudaStream_t st);
 void td_launch_rel_compact(const unsigned char* flag, int n_nodes, int* rel_list, int* n_rel, cudaStream_t st);
 void td_launch_aggregate_h(const float* kbuf, const float* vbuf, const float* e_w, const int* src, const float* q, const float* h_in,
                            float* h_out, int n_nodes, int k, cudaStream_t st);
 void td_launch_aggregate_x(const float* kbuf, const float* v16, const float* e_w, const int* src, const float* q, const float4* xm_in,
                            const int* row_nodes, float4* xm_out, int n_rows, int k, cudaStream_t st);
 void td_launch_aggregate_h_logits(const float* logits, const float* vbuf, const float* e_w, const int* src, const float* h_in, float* h_out,
-                                  int n_nodes, int k, const float* ewm_w, float ewm_b, cudaStream_t st);
+                                  const TdRows& dst, int k, const float* ewm_w, float ewm_b, cudaStream_t st);
 void td_launch_aggregate_x_logits(const float* logits, const float* v16, const float* e_w, const int* src, const float4* xm_in,
                                   const int* row_nodes, float4* xm_out, int n_rows, int k, cudaStream_t st);
 void td_launch_head(const float* h, const int* lig_node, int n_lig, const float* w1t, const float* b1, const float* w2, const float* b2,
