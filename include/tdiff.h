@@ -196,6 +196,30 @@ TDIFF_API int tdiff_sample_seq(tdiff_engine* e, const int32_t* h_time_seq, int n
                                uint64_t seed, float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only,
                                void* stream);
 
+/* Resampled sampling on a time path (an extension beyond the reference, DESIGN.md section 1; RePaint, Lugmayr et al. 2022): the chain
+ * may re-noise the ligand with the forward process between denoising steps.  A time path tau_0, ..., tau_{S-1} has every tau_s in
+ * 0..T-1, tau_0 = T - 1 (t_start while a start is armed, tdiff_set_start), tau_{s+1} != tau_s, tau_1 < tau_0 when S > 1, and
+ * 1 <= S <= TDIFF_PATH_MAX_PER_T * T.  Step s moves the state from t = tau_s to p = tau_{s+1}, or to tau_{S-1} - 1 at the last step.
+ *   Denoising step (p < t): tdiff_sample_seq's step, bit for bit (network at t, unit or jump posterior, fixed rows resampled at p); a
+ *   strictly decreasing path is tdiff_sample_seq's chain.
+ *   Re-noising step (p > t): no network and no time-embedding update.  Every row that is not fixed: x_p = c x_t + d eps with
+ *   c = sqrt(abar_p / abar_t), d = sqrt(1 - abar_p / abar_t) computed in double (log(abar_p / abar_t) = sum_{i = t+1..p} log1p(-beta_i),
+ *   1 - abar_p / abar_t = -expm1 of it), rounded to fp32 once each, each product and the sum rounded once; the type by Gumbel-max over
+ *   log q(v_p | v_t) = log_add_exp(log_onehot(v_t) + lambda, log(1 - e^lambda + 1e-40) - log K), lambda = sum_{i = t+1..p}
+ *   log_alphas_v[i] (log_alphas_v[p] and log_one_minus_alphas_v[p] on a unit step, p = t + 1), log_onehot clamped at 1e-30; with
+ *   pos_only the type stays.  Fixed rows (tdiff_set_fixed) get a sample of q(x_p | x0_f), q(v_p | v0_f) from draw s + 1, as after a
+ *   denoising step.  2 launches.
+ * Noise: step s of either kind reads row s of the tapes [S,Nl,...], or the Philox counters of step s, so a path of S steps uses the
+ * stream of any S-step chain; the fixed tape is [S+1,Nl,...].  Trajectories [S,...], entry s the state after step s: pos_traj and
+ * v_traj the state (fixed rows as held); vt_traj the normalised log-probabilities the type was drawn from; v0_traj the network's
+ * log_softmax at denoising steps, and after a re-noising step a copy of entry s - 1 (the latest network prediction).
+ * Works with tdiff_set_fixed, tdiff_set_start, tapes, pos_only, the time embedding and every layer form.  A NULL or empty path, a
+ * wrong tau_0, equal neighbours, a time outside 0..T-1, an upward first step or a path over the limit -> TDIFF_EINVAL. */
+#define TDIFF_PATH_MAX_PER_T 64
+TDIFF_API int tdiff_sample_path(tdiff_engine* e, const int32_t* h_time_path, int num_steps, const float* d_pos_noise, const float* d_v_uniform,
+                                uint64_t seed, float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only,
+                                void* stream);
+
 /* Start-ligand sampling (an extension beyond the reference, DESIGN.md section 1): arms the next chains to start from the current ligand
  * state (the start ligand x0, v0, centred like any ligand) noised to the start time t_start in 0..T-1, and to run the reverse chain
  * from there; t_start = -1 clears it.  The current ligand state is the one tdiff_set_ligand set or, after a chain, that chain's

@@ -26,7 +26,9 @@
 Result file: `<result_path>/sample.pt` (sample_for_pocket) or `<result_path>/result_{i}.pt` (sample_pockets) = {'data', 'pred_ligand_pos', 'pred_ligand_v', 'pred_ligand_pos_traj', 'pred_ligand_v_traj', 'time'}
 -- the schema scripts/sample_diffusion.py:175-182 writes and scripts/evaluate_diffusion.py:70-76 reads (positions float64, per-sample
 lists; trajectories [steps, atoms, 3]).  With `sample.respaced_steps: n` in the config (an extension beyond the reference) both commands
-run the n-step chain of sampling.respaced_time_seq(T, n) instead of num_steps, and the result also holds 'time_seq'.  Molecule
+run the n-step chain of sampling.respaced_time_seq(T, n) instead of num_steps, and the result also holds 'time_seq'.  With
+`sample.resamplings: r` > 1 (and `sample.jump_length: j`, default 1) sample_for_pocket runs sampling.resampled_time_path over that
+chain, with a --fragment or kept atoms only, and sample.pt also holds 'time_path'; sample_pockets refuses the key.  Molecule
 reconstruction / SDF writing needs RDKit + OpenBabel and stays out of scope."""
 import argparse
 import os
@@ -35,7 +37,7 @@ import sys
 
 import torch
 
-from .config import load_config, sampling_start, sampling_time_seq
+from .config import check_resampling, load_config, sampling_start, sampling_time_path, sampling_time_seq
 from .likelihood import likelihood_time_steps, ligand_nll
 from .pocket import pdb_to_pocket_data
 from .sampling import sample_diffusion_ligand, seed_all
@@ -133,6 +135,7 @@ def sample_pockets(argv):
     a = ap.parse_args(argv)
     config = load_config(a.config)
     sampling_start(config.sample, None, False)      # start ligands are sample_for_pocket's only: refuses sample.start_time
+    check_resampling(config.sample, False)          # so is resampling, which needs held atoms: refuses sample.resamplings
     rank, world, local_rank = tdist.init_from_env()
     device = a.device or 'cuda:%d' % local_rank
     paths = list_pockets(a.pocket_dir, a.pocket_list)
@@ -217,17 +220,25 @@ def sample_for_pocket(argv):
     config = load_config(a.config)
     fragment = load_fragment(a.fragment) if a.fragment else None
     start = load_start_ligand(a.start_ligand) if a.start_ligand else None
+    held = fragment is not None or (start is not None and start[2] is not None and len(start[2]) > 0)
+    check_resampling(config.sample, held)
     seed_all(config.sample.seed)
     model = _load_model(config, a.device)
     start_time, start_seq = sampling_start(config.sample, model.num_timesteps, start is not None)
     time_seq = _time_seq(config, model) if start is None else start_seq
+    T = model.num_timesteps
+    base = time_seq if time_seq is not None else list(range(T - 1, T - 1 - int(config.sample.get('num_steps') or T), -1))
+    time_path = sampling_time_path(config.sample, T, base, held)
     data = pdb_to_pocket_data(a.pdb_path)
     n = a.num_samples if a.num_samples is not None else config.sample.num_samples
     kw = {} if start is None else dict(start_ligand=start[:2], start_time=start_time, keep_atoms=start[2])
+    if time_path is not None:
+        kw['time_path'] = time_path
     outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=a.device,
-                                      num_steps=config.sample.num_steps if time_seq is None else None, pos_only=config.sample.pos_only,
-                                      center_pos_mode=config.sample.center_pos_mode, sample_num_atoms=config.sample.sample_num_atoms,
-                                      fixed_ligand=fragment, time_seq=time_seq, **kw)
+                                      num_steps=config.sample.num_steps if time_seq is None and time_path is None else None,
+                                      pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
+                                      sample_num_atoms=config.sample.sample_num_atoms, fixed_ligand=fragment,
+                                      time_seq=time_seq if time_path is None else None, **kw)
     os.makedirs(a.result_path, exist_ok=True)
     shutil.copyfile(a.config, os.path.join(a.result_path, 'sample.yml'))
     result = build_result(data, outputs)
@@ -241,6 +252,8 @@ def sample_for_pocket(argv):
             result['time_seq'] = time_seq
     elif time_seq is not None:
         result['time_seq'] = time_seq
+    if time_path is not None:
+        result['time_path'] = time_path
     torch.save(result, os.path.join(a.result_path, 'sample.pt'))
     print('Sample done! %d molecules, %.1f s' % (len(outputs[0]), sum(outputs[-1])))
 

@@ -87,6 +87,30 @@ def sampling_start(sample, T, start_ligand):
     return t0, respaced_time_seq(T, n, start=t0)
 
 
+def check_resampling(sample, held):
+    """(r, j) of `sample.resamplings` (default 1: no resampling) and `sample.jump_length` (default 1), an extension beyond the
+    reference's sampling.yml.  ValueError unless both are integers >= 1, and for r > 1 when nothing is `held` (no fragment and no kept
+    atoms): re-noising then only multiplies the cost."""
+    r, j = sample.get('resamplings', 1), sample.get('jump_length', 1)
+    for name, x in (('resamplings', r), ('jump_length', j)):
+        if isinstance(x, bool) or not isinstance(x, int) or x < 1:
+            raise ValueError('sample.%s must be an integer >= 1, got %r' % (name, x))
+    if r > 1 and not held:
+        raise ValueError('sample.resamplings=%d needs held atoms (--fragment, or kept atoms of a --start_ligand): without them '
+                         'resampling only multiplies the cost' % r)
+    return r, j
+
+
+def sampling_time_path(sample, T, base, held):
+    """The resampled time path of check_resampling's (r, j): sampling.resampled_time_path over `base`, the chain's decreasing time
+    sequence (T - 1, ..., 0 when it is None), or None when r = 1."""
+    r, j = check_resampling(sample, held)
+    if r == 1:
+        return None
+    from .sampling import resampled_time_path
+    return resampled_time_path(list(range(T - 1, -1, -1)) if base is None else base, r, j)
+
+
 # Values the sm_90a engine implements; anything else is rejected loudly (SURVEY.md 8(b) "should-reject-clearly").
 _SUPPORTED = dict(model_mean_type=('C0', 'noise'), beta_schedule=('sigmoid', 'linear', 'quad', 'const', 'jsd', 'cosine'),
                   v_beta_schedule=('cosine',), node_indicator=(True,), model_type=('uni_o2',),

@@ -1244,6 +1244,10 @@ void run_step(tdiff_engine* e, cudaStream_t st, const TdStepArgs& base) {
 // keeps almost no bits near t = 0) and a = abar_t / abar_p,
 //   c0 = sqrt(abar_p) (1 - a) / (1 - abar_t),  ct = sqrt(a) (1 - abar_p) / (1 - abar_t),  var = (1 - abar_p) (1 - a) / (1 - abar_t),
 //   lambda = sum_{i = p+1..t} log_alphas_v[i],  l1ma = log(1 - e^lambda + 1e-40)   (oracle/respaced.py:jump_tables).
+// A re-noising step of a time path (p > t, renoise_kernel) reuses the columns: with r = abar_p / abar_t, log r = sum_{i = t+1..p}
+// log1p(-beta_i) from the same prefix sums, c0 <- c = sqrt(r), ct <- d = sqrt(1 - r) (1 - r as -expm1(log r)), logvar <- 0 (unread),
+// la <- lambda = sum_{i = t+1..p} log_alphas_v[i], l1ma <- log(1 - e^lambda + 1e-40); on a unit step up (p = t + 1) la and l1ma are
+// the checkpoint's log_alphas_v[p] and log_one_minus_alphas_v[p] (the reference's q_v_pred_one_timestep)   (oracle/resample.py).
 void seq_tables(const tdiff_engine* e, const int32_t* seq, int S, std::vector<int>& it, std::vector<float>& ft) {
   const float* H = e->host_arena.data();
   auto tab = [&](const float* dev, int t) { return H[(dev - e->arena) + t]; };
@@ -1253,6 +1257,19 @@ void seq_tables(const tdiff_engine* e, const int32_t* seq, int S, std::vector<in
     const int t = seq[s], p = s + 1 < S ? seq[s + 1] : t - 1;
     it[s] = t; it[S + s] = p;
     float* f = ft.data() + s;
+    if (p > t) {
+      const double lr = e->cum_log_a[p] - e->cum_log_a[t];
+      f[0] = (float)sqrt(exp(lr));
+      f[S] = (float)sqrt(-expm1(lr));
+      if (p == t + 1) {
+        f[3 * S] = tab(e->t_la, p); f[4 * S] = tab(e->t_l1ma, p);
+      } else {
+        const double lam = e->cum_log_av[p] - e->cum_log_av[t];
+        f[3 * S] = (float)lam;
+        f[4 * S] = (float)log(1.0 - exp(lam) + 1e-40);
+      }
+      continue;
+    }
     if (p == t - 1) {
       f[0] = tab(e->t_c0, t); f[S] = tab(e->t_ct, t); f[2 * S] = tab(e->t_logvar, t); f[3 * S] = tab(e->t_la, t); f[4 * S] = tab(e->t_l1ma, t);
       continue;
@@ -1268,16 +1285,35 @@ void seq_tables(const tdiff_engine* e, const int32_t* seq, int S, std::vector<in
   }
 }
 
-// The chain of tdiff_sample (time_seq == NULL) and tdiff_sample_seq: eager first step, then one captured step graph replayed.
+// The chain of tdiff_sample (time_seq == NULL), tdiff_sample_seq and tdiff_sample_path (path): eager first step, then one captured
+// denoising-step graph replayed, with a time path's re-noising steps launched between the replays in path order.
 int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const float* d_pos_noise, const float* d_v_uniform, uint64_t seed,
-                 float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only, void* stream) {
+                 float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only, void* stream, bool path = false) {
   if (!e || !e->bound || !e->has_ligand) return set_err(TDIFF_ESTATE, "sample needs bind_batch + set_ligand first");
   const int T = e->cfg.num_timesteps;
   const bool start = e->start_t >= 0;
   if (start && !time_seq)
     return set_err(TDIFF_EINVAL, "a start is armed (tdiff_set_start, t_start=%d): run the chain with tdiff_sample_seq from t_start", e->start_t);
-  if (num_steps < 0 || num_steps > T) return set_err(TDIFF_EINVAL, "num_steps=%d outside 0..%d", num_steps, T);
-  if (time_seq) {
+  if (path) {
+    const char* what = "time path";
+    if (num_steps < 1) return set_err(TDIFF_EINVAL, "%s: empty (num_steps=%d)", what, num_steps);
+    if ((long long)num_steps > (long long)TDIFF_PATH_MAX_PER_T * T)
+      return set_err(TDIFF_EINVAL, "%s: %d steps, more than %d T = %lld", what, num_steps, TDIFF_PATH_MAX_PER_T, (long long)TDIFF_PATH_MAX_PER_T * T);
+    const int t0 = start ? e->start_t : T - 1;
+    if (time_seq[0] != t0)
+      return set_err(TDIFF_EINVAL, start ? "%s: starts at %d, not at the start time t_start = %d" : "%s: starts at %d, not at T - 1 = %d", what,
+                     time_seq[0], t0);
+    for (int s = 1; s < num_steps; ++s) {
+      if (time_seq[s] < 0 || time_seq[s] > T - 1)
+        return set_err(TDIFF_EINVAL, "%s: time %d at step %d outside 0..T-1 = %d", what, time_seq[s], s, T - 1);
+      if (time_seq[s] == time_seq[s - 1]) return set_err(TDIFF_EINVAL, "%s: equal times %d at steps %d and %d", what, time_seq[s], s - 1, s);
+    }
+    if (num_steps > 1 && time_seq[1] > time_seq[0])
+      return set_err(TDIFF_EINVAL, "%s: the first step goes up (%d -> %d); it must evaluate the network", what, time_seq[0], time_seq[1]);
+  } else if (num_steps < 0 || num_steps > T) {
+    return set_err(TDIFF_EINVAL, "num_steps=%d outside 0..%d", num_steps, T);
+  }
+  if (time_seq && !path) {
     if (num_steps < 1) return set_err(TDIFF_EINVAL, "time sequence: empty (num_steps=%d)", num_steps);
     if (start && time_seq[0] != e->start_t)
       return set_err(TDIFF_EINVAL, "time sequence: starts at %d, not at the start time t_start = %d", time_seq[0], e->start_t);
@@ -1350,7 +1386,18 @@ int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const 
   // first step eagerly (module loading, shared-memory attributes), the rest replayed from one captured graph
   run_step(e, st, A);
   int done = 1;
-  if (!eager && num_steps > 2) {
+  // a time path's re-noising steps (p > t): renoise_kernel + advance_step_kernel, no network and no time-embedding update
+  std::vector<char> up(num_steps, 0);
+  int n_denoise = 0;
+  for (int s = 1; s < num_steps; ++s) {
+    up[s] = path && s + 1 < num_steps && time_seq[s + 1] > time_seq[s];
+    n_denoise += !up[s];
+  }
+  auto renoise = [&](cudaStream_t rs) {
+    td_launch_renoise(A, rs);
+    e->launches += 2;
+  };
+  if (!eager && n_denoise >= 2) {
     // fork onto the engine's own stream: capture there (the caller's stream may be the legacy default stream), replay, join back
     cudaStream_t cs = e->own_stream;
     CK(cudaEventRecord(e->ev_fork, st));
@@ -1373,6 +1420,10 @@ int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const 
       return set_err(TDIFF_ECUDA, "CUDA graph capture of the sampling step failed: %s", cudaGetErrorString(ce));
     }
     for (; done < num_steps; ++done) {
+      if (up[done]) {
+        renoise(cs);
+        continue;
+      }
       ce = cudaGraphLaunch(exec, cs);
       if (ce != cudaSuccess) break;
       e->launches += per_step;
@@ -1383,7 +1434,10 @@ int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const 
     cudaGraphDestroy(graph);
     if (ce != cudaSuccess) { delete total; return set_err(TDIFF_ECUDA, "cudaGraphLaunch failed: %s", cudaGetErrorString(ce)); }
   }
-  for (; done < num_steps; ++done) run_step(e, st, A);
+  for (; done < num_steps; ++done) {
+    if (up[done]) renoise(st);
+    else run_step(e, st, A);
+  }
   delete total;
   CK(cudaGetLastError());
   return TDIFF_OK;
@@ -1400,6 +1454,14 @@ extern "C" int tdiff_sample_seq(tdiff_engine* e, const int32_t* h_time_seq, int 
                                 void* stream) {
   if (!h_time_seq) return set_err(TDIFF_EINVAL, "time sequence: null pointer");
   return sample_chain(e, h_time_seq, num_steps, d_pos_noise, d_v_uniform, seed, d_pos_traj, d_v_traj, d_v0_traj, d_vt_traj, pos_only, stream);
+}
+
+extern "C" int tdiff_sample_path(tdiff_engine* e, const int32_t* h_time_path, int num_steps, const float* d_pos_noise, const float* d_v_uniform,
+                                 uint64_t seed, float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only,
+                                 void* stream) {
+  if (!h_time_path) return set_err(TDIFF_EINVAL, "time path: null pointer");
+  return sample_chain(e, h_time_path, num_steps, d_pos_noise, d_v_uniform, seed, d_pos_traj, d_v_traj, d_v0_traj, d_vt_traj, pos_only, stream,
+                      true);
 }
 
 // Likelihood scoring (DESIGN.md section 1): one init launch (x0 / v0 saved, x_t / v_t drawn, t_g / T), the forward, one epilogue launch

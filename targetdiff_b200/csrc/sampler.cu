@@ -269,6 +269,101 @@ void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st) {
   advance_step_kernel<<<1, 1, 0, st>>>(A.step);
 }
 
+// Re-noising step s of a time path (tdiff_sample_path, DESIGN.md section 1): the state moves up from t = seq_t[s] to p = seq_p[s] > t
+// with the forward process, no network.  The step tables hold c = sqrt(abar_p / abar_t) in seq_c0, d = sqrt(1 - abar_p / abar_t) in
+// seq_ct, lambda = log of the type schedule's transition probability t -> p in seq_la and log(1 - e^lambda + 1e-40) in seq_l1ma.  A row
+// that is not fixed: x_p = c x_t + d eps with each product and the sum rounded once (forward_sample's roundings), and a Gumbel-max
+// draw over the unnormalised log q(v_p | v_t) = log_add_exp(log_onehot(v_t) + lambda, l1ma - log K) (q_v_sample's form); with pos_only
+// the type stays.  Fixed rows: q(x_p | x0_f), q(v_p | v0_f) from draw s + 1, as after a denoising step.  The random stream is the
+// denoising step's: row s of the tapes, or counters (a, s, 0, "pst\0") and (a, s, 1 + c/4, "vuni").  Trajectories: pos_traj / v_traj
+// the new state, vt_traj the normalised log q(v_p | v_t), v0_traj a copy of entry s - 1 (the latest network prediction).
+template <bool kFixed>
+__global__ void renoise_kernel(TdStepArgs A) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= A.n_lig) return;
+  const int s = *A.step;
+  const int p = A.seq_p[s];
+  const int K = A.n_classes;
+  const bool fixed = kFixed && A.fix_mask[a];
+  const uint2 key = make_uint2((unsigned)A.seed, (unsigned)(A.seed >> 32));
+  float4 xn;
+  int vnew = A.lig_v[a];
+  if (!fixed) {
+    float nz[3];
+    if (A.pos_noise) {
+      const float* pn = A.pos_noise + ((size_t)s * A.n_lig + a) * 3;
+      nz[0] = pn[0]; nz[1] = pn[1]; nz[2] = pn[2];
+    } else {
+      const uint4 r0 = philox4x32_10(make_uint4((unsigned)a, (unsigned)s, 0u, 0x70737400u), key);
+      const float u0 = 1.0f - u01(r0.x), u1 = u01(r0.y), u2 = 1.0f - u01(r0.z), u3 = u01(r0.w);
+      const float ra = sqrtf(-2.0f * logf(u0)), rb = sqrtf(-2.0f * logf(u2));
+      nz[0] = ra * cospif(2.0f * u1); nz[1] = ra * sinpif(2.0f * u1); nz[2] = rb * cospif(2.0f * u3);
+    }
+    const float4 xt = A.lig_pos[a];
+    const float c = A.seq_c0[s], d = A.seq_ct[s];
+    xn.x = __fadd_rn(__fmul_rn(c, xt.x), __fmul_rn(d, nz[0]));
+    xn.y = __fadd_rn(__fmul_rn(c, xt.y), __fmul_rn(d, nz[1]));
+    xn.z = __fadd_rn(__fmul_rn(c, xt.z), __fmul_rn(d, nz[2]));
+    xn.w = 1.0f;
+  } else {
+    fixed_sample(A, a, s + 1, p, xn, vnew);
+  }
+  if (!A.pos_only) {
+    const float la = A.seq_la[s], l1ma = A.seq_l1ma[s] - A.log_k;
+    const float log_eps = -69.07755279f;                                   // logf(1e-30f): index_to_log_onehot's clamp
+    const int vcur = A.lig_v[a];
+    float lq[TD_CMAX];
+    float mx = -INFINITY;
+    for (int c = 0; c < K; ++c) {
+      lq[c] = log_add_exp_f(((c == vcur) ? 0.0f : log_eps) + la, l1ma);
+      mx = fmaxf(mx, lq[c]);
+    }
+    float se = 0.0f;
+    for (int c = 0; c < K; ++c) se += expf(lq[c] - mx);
+    const float lse = mx + logf(se);                                       // torch.logsumexp
+    float* ot = A.vt_traj ? A.vt_traj + ((size_t)s * A.n_lig + a) * K : nullptr;
+    float* o0 = A.v0_traj ? A.v0_traj + ((size_t)s * A.n_lig + a) * K : nullptr;
+    const float* p0 = o0 ? o0 - (size_t)A.n_lig * K : nullptr;
+    float best = -INFINITY;
+    int vbest = 0;
+    for (int c0 = 0; c0 < K; c0 += 4) {
+      float u[4];
+      if (A.v_uniform) {
+        const float* vu = A.v_uniform + ((size_t)s * A.n_lig + a) * K;
+        for (int j = 0; j < 4 && c0 + j < K; ++j) u[j] = vu[c0 + j];
+      } else {
+        const uint4 r = philox4x32_10(make_uint4((unsigned)a, (unsigned)s, 1u + (unsigned)(c0 >> 2), 0x76756e69u), key);
+        u[0] = u01(r.x); u[1] = u01(r.y); u[2] = u01(r.z); u[3] = u01(r.w);
+      }
+      for (int j = 0; j < 4 && c0 + j < K; ++j) {
+        const int c = c0 + j;
+        const float sc = -logf(-logf(u[j] + 1e-30f) + 1e-30f) + lq[c];
+        if (sc > best) { best = sc; vbest = c; }
+        if (ot) ot[c] = lq[c] - lse;
+        if (o0) o0[c] = p0[c];
+      }
+    }
+    if (!fixed) vnew = vbest;
+    A.lig_v[a] = vnew;
+  }
+  A.lig_pos[a] = xn;
+  if (A.pos_traj) {
+    const float4 off = A.offset[A.lig_graph[a]];
+    float* o = A.pos_traj + ((size_t)s * A.n_lig + a) * 3;
+    o[0] = xn.x + off.x; o[1] = xn.y + off.y; o[2] = xn.z + off.z;
+  }
+  if (A.v_traj) A.v_traj[(size_t)s * A.n_lig + a] = (long long)vnew;
+}
+
+void td_launch_renoise(const TdStepArgs& A, cudaStream_t st) {
+  if (A.n_lig > 0) {
+    const int grid = (A.n_lig + 127) / 128;
+    if (A.fix_mask) renoise_kernel<true><<<grid, 128, 0, st>>>(A);
+    else renoise_kernel<false><<<grid, 128, 0, st>>>(A);
+  }
+  advance_step_kernel<<<1, 1, 0, st>>>(A.step);
+}
+
 // fixed rows <- q(x_{T-1} | x0_f), q(v_{T-1} | v0_f) from draw 0, once before the first step of a chain
 __global__ void fixed_init_kernel(TdStepArgs A) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;

@@ -32,7 +32,8 @@ struct TdStepArgs {
   const float* ac;                 // alphas_cumprod [T]
   const float* fix_pos_noise;      // fixed-atom tape [S+1,Nl,3] or NULL (Philox, FIX_POS domain)
   const float* fix_v_uniform;      // fixed-atom tape [S+1,Nl,K] or NULL (Philox, FIX_TYPE domain)
-  // respaced chain (tdiff_sample_seq); seq_t == NULL: the default chain, t = t_start - step, and the kernel takes that path only
+  // respaced chain (tdiff_sample_seq) or time path (tdiff_sample_path); seq_t == NULL: the default chain, t = t_start - step, and the
+  // kernel takes that path only.  A re-noising step (p > t) keeps c, d, lambda, l1ma in seq_c0, seq_ct, seq_la, seq_l1ma (renoise_kernel)
   const int* seq_t;                // [S] tau_s, the time the network sees at step s
   const int* seq_p;                // [S] the time step s moves to: tau_{s+1}, or tau_{S-1} - 1 at the last step
   const float *seq_c0, *seq_ct, *seq_logvar;   // [S] position posterior of the jump t -> p (the checkpoint's tables at t on unit steps)
@@ -67,6 +68,7 @@ struct TdLikelihoodArgs {
 };
 
 void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st);
+void td_launch_renoise(const TdStepArgs& A, cudaStream_t st);
 void td_launch_fixed_init(const TdStepArgs& A, cudaStream_t st);
 void td_launch_start_init(const TdStepArgs& A, cudaStream_t st);
 void td_launch_likelihood_init(const TdLikelihoodArgs& L, cudaStream_t st);

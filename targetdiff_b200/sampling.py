@@ -31,14 +31,21 @@ start=t0)).  Every sample has the start ligand's n atoms (`sample_num_atoms` is 
 made.  `keep_atoms` (indices into the start ligand) become fixed rows, held to the forward process of their start positions and types.
 Under rng='cpu' each batch draws, in this order, the start tape randn(Nl, 3), rand(Nl, K) (the uniforms skipped under pos_only), the
 step tape in the reference's interleaved order, and with kept atoms the fixed tape randn(S+1, Nl, 3), rand(S+1, Nl, K) (the uniforms
-skipped under pos_only).  With pos_only the types are the start ligand's.  Sample quality from a start ligand has not been measured."""
+skipped under pos_only).  With pos_only the types are the start ligand's.  Sample quality from a start ligand has not been measured.
+
+Resampled sampling (an extension beyond the reference, DESIGN.md section 1; RePaint, Lugmayr et al. 2022).  `time_path` (e.g.
+`resampled_time_path(base, resamplings=r, jump_length=j)`) runs a time path whose steps may go up: a re-noising step draws the whole
+state back up with the forward process, so that the free atoms are denoised again next to the held fragment or kept atoms
+(ScorePosNet3D.sample_diffusion(time_path=...)).  Not with `time_seq`; with a start ligand the path begins at the start time.  Under
+rng='cpu' the draws are those of a time_seq of S = len(time_path) steps.  Whether resampling improves the molecules has not been
+measured."""
 import time
 
 import numpy as np
 import torch
 
 from . import atom_num
-from .score_model import check_time_seq, log_sample_categorical
+from .score_model import check_time_path, check_time_seq, log_sample_categorical
 
 
 def seed_all(seed):
@@ -70,7 +77,32 @@ def respaced_time_seq(T, n, start=None):
     return seq
 
 
-def _check_start(model, start_ligand, start_time, keep_atoms, fixed_ligand):
+def resampled_time_path(base, resamplings=1, jump_length=1):
+    """The RePaint time path (Lugmayr et al. 2022) over a strictly decreasing base sequence b_0 > ... > b_{n-1} >= 0 (the default chain,
+    a respaced_time_seq, or one from a start time), for ScorePosNet3D.sample_diffusion(time_path=...).  The base indices fall into blocks
+    [k j, e] with e = min(k j + j, n - 1); each block is denoised from b_{kj} down to b_e, then `resamplings` - 1 times re-noised in one
+    step from b_e back up to b_{kj} and denoised again; the path ends with the last step at b_{n-1}.  That is r (n - 1) + 1 denoising
+    and (r - 1) ceil((n - 1) / j) re-noising steps; r = 1 gives the base itself."""
+    b = [int(x) for x in (base.tolist() if hasattr(base, 'tolist') else base)]
+    r, j = int(resamplings), int(jump_length)
+    if not b or any(y >= x for x, y in zip(b, b[1:])) or b[-1] < 0:
+        raise ValueError('the base of a resampled time path must be a non-empty strictly decreasing sequence of times >= 0')
+    if r < 1:
+        raise ValueError('resamplings must be >= 1, got %d' % r)
+    if j < 1:
+        raise ValueError('jump_length must be >= 1, got %d' % j)
+    n = len(b)
+    path = [b[0]]
+    for k0 in range(0, n - 1, j):
+        e = min(k0 + j, n - 1)
+        for rep in range(r):
+            if rep > 0:
+                path.append(b[k0])                                      # one re-noising step from b_e back up to b_{kj}
+            path += b[k0 + 1:e + 1]
+    return path
+
+
+def _check_start(model,start_ligand, start_time, keep_atoms, fixed_ligand):
     """(pos [n,3] float32, v [n] int64, t0, keep [k] int64) of a start ligand, or None without one; ValueError for what
     sample_diffusion_ligand refuses."""
     if start_ligand is None:
@@ -115,11 +147,17 @@ def _split(arr, cum, n_data):
 
 def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cuda:0', num_steps=None, pos_only=False,
                             center_pos_mode='protein', sample_num_atoms='prior', rng='device', fixed_ligand=None, time_seq=None,
-                            start_ligand=None, start_time=None, keep_atoms=None):
+                            start_ligand=None, start_time=None, keep_atoms=None, time_path=None):
     if rng not in ('device', 'cpu'):
         raise ValueError("rng must be 'device' or 'cpu'")
     start = _check_start(model, start_ligand, start_time, keep_atoms, fixed_ligand)
-    if start is not None and time_seq is None:
+    if time_path is not None:
+        if time_seq is not None:
+            raise ValueError('time_path cannot be combined with time_seq')
+        time_path = check_time_path(time_path, model.num_timesteps, start=None if start is None else start[2])
+        if num_steps is not None and int(num_steps) != len(time_path):
+            raise ValueError('num_steps=%d disagrees with a time_path of %d steps' % (int(num_steps), len(time_path)))
+    elif start is not None and time_seq is None:
         time_seq = list(range(start[2], -1, -1))
     if time_seq is not None:
         time_seq = check_time_seq(time_seq, model.num_timesteps, start=None if start is None else start[2])
@@ -174,6 +212,8 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
             # of the pocket has the same centre)
             n_lig = len(batch_ligand)
             extra = {} if time_seq is None else {'time_seq': time_seq}
+            if time_path is not None:
+                extra['time_path'] = time_path
             if start is not None:                                       # the clean start ligand; the engine noises it to t0
                 init_ligand_pos = start[0].to(device).repeat(n_data, 1)
                 init_ligand_v = start[1].to(device).repeat(n_data)
@@ -192,7 +232,8 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
                     init_ligand_v = log_sample_categorical(uniform_logits).to(device)
             tape = None
             if rng == 'cpu':
-                S = len(time_seq) if time_seq is not None else model.num_timesteps if num_steps is None else int(num_steps)
+                S = len(time_seq) if time_seq is not None else len(time_path) if time_path is not None else \
+                    model.num_timesteps if num_steps is None else int(num_steps)
                 pn = torch.empty(S, n_lig, 3)
                 vu = torch.zeros(S, n_lig, model.num_classes)
                 for st in range(S):                                     # the reference's interleaved draw order

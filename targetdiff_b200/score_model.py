@@ -192,6 +192,37 @@ def check_time_seq(time_seq, T, start=None):
     return seq
 
 
+PATH_MAX_PER_T = 64          # TDIFF_PATH_MAX_PER_T (include/tdiff.h): a time path has at most 64 T steps
+
+
+def check_time_path(time_path, T, start=None):
+    """`time_path` as a list of ints, or ValueError unless it is a time path (DESIGN.md section 1): every tau_s in 0..T-1, tau_0 = T - 1
+    (the start time `start` with a start ligand), tau_{s+1} != tau_s, tau_1 < tau_0 when S > 1 (the first step evaluates the network),
+    1 <= S <= PATH_MAX_PER_T * T."""
+    path = [int(x) for x in (time_path.tolist() if hasattr(time_path, 'tolist') else time_path)]
+    if not path:
+        raise ValueError('time_path is empty')
+    if len(path) > PATH_MAX_PER_T * T:
+        raise ValueError('time_path has %d steps, more than %d T = %d' % (len(path), PATH_MAX_PER_T, PATH_MAX_PER_T * T))
+    if start is None:
+        if path[0] != T - 1:
+            raise ValueError('time_path must start at T - 1 = %d, not %d' % (T - 1, path[0]))
+    else:
+        if not 0 <= int(start) <= T - 1:
+            raise ValueError('start time %d outside 0..T-1 = %d' % (int(start), T - 1))
+        if path[0] != int(start):
+            raise ValueError('time_path must start at the start time %d, not %d' % (int(start), path[0]))
+    bad = [x for x in path if not 0 <= x <= T - 1]
+    if bad:
+        raise ValueError('time_path has a time %d outside 0..T-1 = %d' % (bad[0], T - 1))
+    for s, (a, b) in enumerate(zip(path, path[1:])):
+        if a == b:
+            raise ValueError('time_path repeats time %d at steps %d and %d' % (a, s, s + 1))
+    if len(path) > 1 and path[1] > path[0]:
+        raise ValueError('time_path goes up at its first step (%d -> %d); the first step must evaluate the network' % (path[0], path[1]))
+    return path
+
+
 def _counts_from_batch(batch, name):
     """Per-graph atom counts from a sorted PyG-style batch vector (host list)."""
     if batch.numel() == 0:
@@ -381,7 +412,8 @@ class ScorePosNet3D(nn.Module):
     @torch.no_grad()
     def sample_diffusion(self, protein_pos, protein_v, batch_protein, init_ligand_pos, init_ligand_v, batch_ligand,
                          num_steps=None, center_pos_mode=None, pos_only=False, noise_tape=None, seed=None, return_traj=True,
-                         stack_traj=False, fixed_mask=None, fixed_noise_tape=None, time_seq=None, start_time=None, start_noise_tape=None):
+                         stack_traj=False, fixed_mask=None, fixed_noise_tape=None, time_seq=None, start_time=None, start_noise_tape=None,
+                         time_path=None):
         """The reverse-diffusion chain (reference models/molopt_score_model.py:633-703), executed entirely by libtdiff.so.
 
         Extensions over the reference signature (all optional): `noise_tape=(pos_noise [S,Nl,3], v_uniform [S,Nl,K])`
@@ -404,13 +436,27 @@ class ScorePosNet3D(nn.Module):
         start ligand; before the first step every row that is not fixed is replaced by a sample of q(x_t0 | x0), q(v_t0 | v0) (the types
         are kept with pos_only), fixed rows get their sample at t0, and the chain runs from t0: `time_seq` defaults to t0, t0 - 1, ..., 0
         (t0 + 1 steps) and must begin at t0.  `start_noise_tape=(pos_noise [Nl,3], v_uniform [Nl,K])` replaces the start draw (v_uniform
-        may be None with pos_only); it is required with `noise_tape` and not allowed without it.  Sample quality is not measured."""
+        may be None with pos_only); it is required with `noise_tape` and not allowed without it.  Sample quality is not measured.
+
+        Resampled sampling (DESIGN.md section 1): `time_path` (check_time_path; e.g. sampling.resampled_time_path) runs a path whose
+        steps may go up: step s moves the state from tau_s to p = tau_{s+1} (tau_{S-1} - 1 at the last step); a denoising step (p < tau_s)
+        is time_seq's step, a re-noising step (p > tau_s) draws the state from the forward process q(x_p | x_t), q(v_p | v_t) without the
+        network, and fixed rows are resampled at p after either.  Not with `time_seq`; it begins at the start time with `start_time`.
+        Tapes are [S, ...] (fixed tape [S+1, ...]), trajectories [S, ...]; after a re-noising step v0_traj repeats the entry before and
+        vt_traj holds the normalised log q(v_p | v_t).  Sample quality is not measured."""
         T = self.num_timesteps
+        if time_path is not None:
+            if time_seq is not None:
+                raise ValueError('time_path cannot be combined with time_seq')
+            time_path = check_time_path(time_path, T, start=start_time)
+            if num_steps is not None and int(num_steps) != len(time_path):
+                raise ValueError('num_steps=%d disagrees with a time_path of %d steps' % (int(num_steps), len(time_path)))
+            num_steps = len(time_path)
         if start_time is not None:
             t0 = int(start_time)
             if not 0 <= t0 <= T - 1:
                 raise ValueError('start_time %d outside 0..T-1 = %d' % (t0, T - 1))
-            if time_seq is None:
+            if time_seq is None and time_path is None:
                 time_seq = list(range(t0, -1, -1))
             if (start_noise_tape is None) != (noise_tape is None):
                 raise ValueError('start_noise_tape is required with noise_tape, and not allowed without it')
@@ -478,7 +524,10 @@ class ScorePosNet3D(nn.Module):
             if not pos_only:
                 v0_traj = torch.empty(S, Nl, K, device=dev)
                 vt_traj = torch.empty(S, Nl, K, device=dev)
-        if time_seq is None:
+        if time_path is not None:
+            _lib.check(lib.tdiff_sample_path(eng, _lib.i32_array(time_path), S, _ptr(pos_noise), _ptr(v_uniform), ctypes.c_uint64(seed),
+                                             _ptr(pos_traj), _ptr(v_traj), _ptr(v0_traj), _ptr(vt_traj), int(bool(pos_only)), st))
+        elif time_seq is None:
             _lib.check(lib.tdiff_sample(eng, S, _ptr(pos_noise), _ptr(v_uniform), ctypes.c_uint64(seed), _ptr(pos_traj), _ptr(v_traj),
                                         _ptr(v0_traj), _ptr(vt_traj), int(bool(pos_only)), st))
         else:
