@@ -220,6 +220,20 @@ TDIFF_API int tdiff_sample_path(tdiff_engine* e, const int32_t* h_time_path, int
                                 uint64_t seed, float* d_pos_traj, int64_t* d_v_traj, float* d_v0_traj, float* d_vt_traj, int pos_only,
                                 void* stream);
 
+/* Clash guidance (an extension beyond the reference, DESIGN.md section 1): at every denoising step of every following chain
+ * (tdiff_sample, tdiff_sample_seq, the denoising steps of tdiff_sample_path), the step's x0 prediction y of each ligand atom (after the
+ * 'noise' mean type's conversion; centred frame) is replaced by
+ *   y + strength * sum_p (radius - d) (y - x_p) / d,   d = |y - x_p|,
+ * over the protein atoms p of the same graph at their bound positions x_p with 0 < d < radius -- y - (strength / 2) grad E(y) for
+ * E(y) = sum_p max(0, radius - |y - x_p|)^2.  An atom without such a pair keeps y bit for bit.  The step then runs unchanged on the
+ * guided prediction (posterior, noise, types, fixed-row overwrite, trajectories); fixed rows are guided and then overwritten as before.
+ * fp32; every sum runs over the graph's own protein atoms in bind order, so a graph gets the same bits in any batch.  No random numbers
+ * are drawn.  One more launch per denoising step; re-noising steps, tdiff_forward, tdiff_forward_blocks and tdiff_likelihood_terms
+ * ignore the setting.  strength == 0 turns guidance off (radius is then ignored); strength > 0 needs a finite radius > 0 (Angstrom).  A
+ * negative or non-finite strength, or a bad radius with strength > 0 -> TDIFF_EINVAL and the previous setting stays.  The setting
+ * belongs to the handle: it refers to no batch rows, so it survives tdiff_bind_batch.  Off on a new handle. */
+TDIFF_API int tdiff_set_clash_guidance(tdiff_engine* e, float radius, float strength);
+
 /* Start-ligand sampling (an extension beyond the reference, DESIGN.md section 1): arms the next chains to start from the current ligand
  * state (the start ligand x0, v0, centred like any ligand) noised to the start time t_start in 0..T-1, and to run the reverse chain
  * from there; t_start = -1 clears it.  The current ligand state is the one tdiff_set_ligand set or, after a chain, that chain's

@@ -47,3 +47,22 @@ def check_stability(positions, atom_type, debug=False, hs=False, return_nr_bonds
     if return_nr_bonds:
         return bool(ms[0]), int(ns[0]), int(n[0]), nb
     return bool(ms[0]), int(ns[0]), int(n[0])
+
+
+def protein_contacts(ligand_pos, protein_pos, batch_ligand, batch_protein, radius):
+    """Per molecule g: (number of ligand atoms of g with a protein atom of g closer than `radius`, the smallest ligand-protein
+    distance within g, inf without pairs) as (int64 [B], float64 [B]) tensors on the CPU, B = the number of molecules.  Computed in
+    torch in float64 on the CPU, for the clash-guidance tests and timing tool; it counts contacts, it is not a quality metric."""
+    lp, pp = torch.as_tensor(ligand_pos).detach().cpu().double(), torch.as_tensor(protein_pos).detach().cpu().double()
+    bl, bp = torch.as_tensor(batch_ligand).detach().cpu().long(), torch.as_tensor(batch_protein).detach().cpu().long()
+    B = int(max(int(bl.max()) if bl.numel() else -1, int(bp.max()) if bp.numel() else -1)) + 1
+    n_close = torch.zeros(B, dtype=torch.int64)
+    d_min = torch.full((B,), float('inf'), dtype=torch.float64)
+    for g in range(B):
+        a, p = lp[bl == g], pp[bp == g]
+        if len(a) == 0 or len(p) == 0:
+            continue
+        d = torch.cdist(a, p, compute_mode='donot_use_mm_for_euclid_dist').min(dim=1).values
+        n_close[g] = int((d < radius).sum())
+        d_min[g] = float(d.min())
+    return n_close, d_min

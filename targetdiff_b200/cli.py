@@ -28,7 +28,9 @@ Result file: `<result_path>/sample.pt` (sample_for_pocket) or `<result_path>/res
 lists; trajectories [steps, atoms, 3]).  With `sample.respaced_steps: n` in the config (an extension beyond the reference) both commands
 run the n-step chain of sampling.respaced_time_seq(T, n) instead of num_steps, and the result also holds 'time_seq'.  With
 `sample.resamplings: r` > 1 (and `sample.jump_length: j`, default 1) sample_for_pocket runs sampling.resampled_time_path over that
-chain, with a --fragment or kept atoms only, and sample.pt also holds 'time_path'; sample_pockets refuses the key.  Molecule
+chain, with a --fragment or kept atoms only, and sample.pt also holds 'time_path'; sample_pockets refuses the key.  With
+`sample.clash_strength: lambda` > 0 and `sample.clash_radius: rho` (config.sample_clash_guidance; strength 0, the default, is off) both
+commands run clash guidance (ScorePosNet3D.sample_diffusion), and the result also holds 'clash_guidance': {'radius', 'strength'}.  Molecule
 reconstruction / SDF writing needs RDKit + OpenBabel and stays out of scope."""
 import argparse
 import os
@@ -37,7 +39,7 @@ import sys
 
 import torch
 
-from .config import check_resampling, load_config, sampling_start, sampling_time_path, sampling_time_seq
+from .config import check_resampling, load_config, sample_clash_guidance, sampling_start, sampling_time_path, sampling_time_seq
 from .likelihood import likelihood_time_steps, ligand_nll
 from .pocket import pdb_to_pocket_data
 from .sampling import sample_diffusion_ligand, seed_all
@@ -52,6 +54,13 @@ def build_result(data, outputs):
     pred_pos, pred_v, pred_pos_traj, pred_v_traj, pred_v0_traj, pred_vt_traj, time_list = outputs
     return {'data': data, 'pred_ligand_pos': pred_pos, 'pred_ligand_v': pred_v, 'pred_ligand_pos_traj': pred_pos_traj,
             'pred_ligand_v_traj': pred_v_traj, 'time': time_list}
+
+
+def add_clash_guidance(result, radius, strength):
+    """Record a clash-guidance setting in a result dict; nothing when guidance is off, so the file is as without it."""
+    if strength > 0:
+        result['clash_guidance'] = {'radius': radius, 'strength': strength}
+    return result
 
 
 def _load_model(config, device, rank=0):
@@ -136,6 +145,7 @@ def sample_pockets(argv):
     config = load_config(a.config)
     sampling_start(config.sample, None, False)      # start ligands are sample_for_pocket's only: refuses sample.start_time
     check_resampling(config.sample, False)          # so is resampling, which needs held atoms: refuses sample.resamplings
+    clash_radius, clash_strength = sample_clash_guidance(config.sample)
     rank, world, local_rank = tdist.init_from_env()
     device = a.device or 'cuda:%d' % local_rank
     paths = list_pockets(a.pocket_dir, a.pocket_list)
@@ -153,8 +163,9 @@ def sample_pockets(argv):
         data = pdb_to_pocket_data(paths[i])
         outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=device, num_steps=num_steps,
                                           pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
-                                          sample_num_atoms=config.sample.sample_num_atoms, time_seq=time_seq)
-        result = build_result(data, outputs)
+                                          sample_num_atoms=config.sample.sample_num_atoms, time_seq=time_seq,
+                                          clash_radius=clash_radius, clash_strength=clash_strength)
+        result = add_clash_guidance(build_result(data, outputs), clash_radius, clash_strength)
         if time_seq is not None:
             result['time_seq'] = time_seq
         torch.save(result, os.path.join(a.result_path, 'result_%d.pt' % i))
@@ -222,6 +233,7 @@ def sample_for_pocket(argv):
     start = load_start_ligand(a.start_ligand) if a.start_ligand else None
     held = fragment is not None or (start is not None and start[2] is not None and len(start[2]) > 0)
     check_resampling(config.sample, held)
+    clash_radius, clash_strength = sample_clash_guidance(config.sample)
     seed_all(config.sample.seed)
     model = _load_model(config, a.device)
     start_time, start_seq = sampling_start(config.sample, model.num_timesteps, start is not None)
@@ -238,10 +250,11 @@ def sample_for_pocket(argv):
                                       num_steps=config.sample.num_steps if time_seq is None and time_path is None else None,
                                       pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
                                       sample_num_atoms=config.sample.sample_num_atoms, fixed_ligand=fragment,
-                                      time_seq=time_seq if time_path is None else None, **kw)
+                                      time_seq=time_seq if time_path is None else None, clash_radius=clash_radius,
+                                      clash_strength=clash_strength, **kw)
     os.makedirs(a.result_path, exist_ok=True)
     shutil.copyfile(a.config, os.path.join(a.result_path, 'sample.yml'))
-    result = build_result(data, outputs)
+    result = add_clash_guidance(build_result(data, outputs), clash_radius, clash_strength)
     if fragment is not None:
         result['fixed_ligand_atoms'] = int(fragment[1].shape[0])
     if start is not None:

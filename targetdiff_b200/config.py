@@ -1,4 +1,7 @@
 """Configuration surface of the sampling path (reference utils/misc.py:23-25, configs/training.yml, configs/sampling.yml)."""
+import math
+import numbers
+
 import yaml
 
 
@@ -99,6 +102,30 @@ def check_resampling(sample, held):
         raise ValueError('sample.resamplings=%d needs held atoms (--fragment, or kept atoms of a --start_ligand): without them '
                          'resampling only multiplies the cost' % r)
     return r, j
+
+
+def check_clash_guidance(radius, strength):
+    """(radius, strength) as floats, or ValueError unless they are a clash-guidance setting (DESIGN.md section 1): strength finite and
+    >= 0, 0 turning guidance off (radius is then ignored and returned as None); with strength > 0 a finite radius > 0 in Angstrom.
+    The same refusals as tdiff_set_clash_guidance.  ScorePosNet3D.sample_diffusion and the config keys (sample_clash_guidance) use it."""
+    if isinstance(strength, bool) or not isinstance(strength, numbers.Real):
+        raise ValueError('clash_strength must be a number, got %r' % (strength,))
+    strength = float(strength)
+    if not math.isfinite(strength) or strength < 0:
+        raise ValueError('clash_strength must be finite and >= 0 (0 turns guidance off), got %r' % strength)
+    if strength == 0:
+        return None, 0.0
+    if radius is None:
+        raise ValueError('clash_strength=%g needs a clash_radius' % strength)
+    if isinstance(radius, bool) or not isinstance(radius, numbers.Real) or not math.isfinite(float(radius)) or float(radius) <= 0:
+        raise ValueError('clash_radius must be a finite number > 0 (Angstrom), got %r' % (radius,))
+    return float(radius), strength
+
+
+def sample_clash_guidance(sample):
+    """(radius, strength) of `sample.clash_radius` and `sample.clash_strength` (an extension beyond the reference's sampling.yml):
+    strength defaults to 0 (off) and the radius has no default.  check_clash_guidance's refusals, as ValueError."""
+    return check_clash_guidance(sample.get('clash_radius'), sample.get('clash_strength', 0.0))
 
 
 def sampling_time_path(sample, T, base, held):

@@ -144,6 +144,10 @@ struct tdiff_engine {
   // likelihood scoring (tdiff_likelihood_terms): t_g, k_g [B] int32 | the clean ligand x0 [Nl] float4, v0 [Nl] int, kept during the call
   DevBuf lk_buf, lk_x0, lk_v0;
   std::vector<int32_t> lk_host;
+  // clash guidance (tdiff_set_clash_guidance): off while clash_strength == 0; a handle setting, kept across tdiff_bind_batch.  guided
+  // [N] float4: the guided x0 predictions of a step at the ligand rows (clash_guidance_kernel), the epilogue's xm_final
+  float clash_radius = 0.f, clash_strength = 0.f;
+  DevBuf guided;
   DevBuf stage[8];   // staging for tdiff_sample_host
   // ---- instrumentation
   cudaStream_t own_stream = nullptr;   // capture stream (the caller's stream may be the legacy default stream, which cannot capture)
@@ -693,7 +697,7 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   int bad = 0;
   bad |= e->node_ptr.ensure((B + 1) * 4) | e->prot_ptr.ensure((B + 1) * 4) | e->prot_node.ensure(Np * 4 + 4) | e->prot_graph.ensure(Np * 4 + 4);
   bad |= e->lig_node.ensure(Nl * 4 + 4) | e->lig_graph.ensure(Nl * 4 + 4) | e->node_lig.ensure(N * 4);
-  bad |= e->xm0.ensure(N * 16) | e->xm1.ensure(N * 16) | e->offset.ensure((size_t)B * 16);
+  bad |= e->xm0.ensure(N * 16) | e->xm1.ensure(N * 16) | e->guided.ensure(N * 16) | e->offset.ensure((size_t)B * 16);
   bad |= e->h0.ensure(N * TD_H * 4) | e->h.ensure(N * TD_H * 4) | e->P.ensure((size_t)(N + 1) * TD_NPROJ * 4) | e->q.ensure(N * TD_H * 4);
   bad |= e->src.ensure(slots * 4) | e->src_prev.ensure(slots * 4) | e->etype.ensure(slots) | e->e_w.ensure(slots * 4) | e->dist.ensure(slots * 4);
   // class-sorted destination lists (v4 edge kernel): each class padded so that its rows end on a 128-row tile boundary
@@ -1234,6 +1238,16 @@ void run_step(tdiff_engine* e, cudaStream_t st, const TdStepArgs& base) {
   e->restrict_last = false;
   TdStepArgs A = base;
   A.xm_final = e->final_buf ? e->xm1.as<float4>() : e->xm0.as<float4>();
+  if (e->clash_strength > 0.f) {   // clash guidance (DESIGN.md section 1): the epilogue reads the guided, already converted x0
+    TdGuideArgs G;
+    G.node_ptr = e->node_ptr.as<int>(); G.prot_ptr = e->prot_ptr.as<int>();
+    G.prot_xm = e->xm0.as<float4>();      // protein rows: the bound positions place_protein_kernel wrote; no kernel writes them later
+    G.guided = e->guided.as<float4>(); G.radius = e->clash_radius; G.strength = e->clash_strength;
+    td_launch_clash_guidance(A, G, e->B, st);
+    A.xm_final = e->guided.as<float4>();
+    A.mean_noise = 0;
+    e->launches += 1;
+  }
   td_launch_step_epilogue(A, st);
   e->launches += 2;
 }
@@ -1462,6 +1476,17 @@ extern "C" int tdiff_sample_path(tdiff_engine* e, const int32_t* h_time_path, in
   if (!h_time_path) return set_err(TDIFF_EINVAL, "time path: null pointer");
   return sample_chain(e, h_time_path, num_steps, d_pos_noise, d_v_uniform, seed, d_pos_traj, d_v_traj, d_v0_traj, d_vt_traj, pos_only, stream,
                       true);
+}
+
+extern "C" int tdiff_set_clash_guidance(tdiff_engine* e, float radius, float strength) {
+  if (!e) return set_err(TDIFF_EINVAL, "set_clash_guidance: null engine");
+  if (!isfinite(strength) || strength < 0.f)
+    return set_err(TDIFF_EINVAL, "set_clash_guidance: strength=%g must be finite and >= 0 (0 turns guidance off)", (double)strength);
+  if (strength > 0.f && !(isfinite(radius) && radius > 0.f))
+    return set_err(TDIFF_EINVAL, "set_clash_guidance: radius=%g must be finite and > 0 when strength > 0", (double)radius);
+  e->clash_strength = strength;
+  e->clash_radius = strength > 0.f ? radius : 0.f;
+  return TDIFF_OK;
 }
 
 // Likelihood scoring (DESIGN.md section 1): one init launch (x0 / v0 saved, x_t / v_t drawn, t_g / T), the forward, one epilogue launch

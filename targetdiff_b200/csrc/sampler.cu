@@ -139,9 +139,24 @@ __device__ __forceinline__ void fixed_sample(const TdStepArgs& A, int a, int d, 
   forward_sample<TdFixedSource>(A, a, d, tm, x, v);
 }
 
+// The step's x0 prediction of ligand row `a` at network time t, centred frame: the node array's row in C0 mode; in 'noise' mode
+// x0 = sqrt(1/ac) x_t - sqrt(1/ac - 1) (pred - x_t)   (reference :419-422,663-666).  Shared by step_epilogue_kernel and
+// clash_guidance_kernel, so that a row guidance leaves alone has the same bits in a guided and an unguided step.
+__device__ __forceinline__ float4 td_pred_x0(const TdStepArgs& A, int a, int t, const float4& xt) {
+  float4 x0 = A.xm_final[A.lig_node[a]];
+  if (A.mean_noise) {
+    const float ra = A.sra[t], rm = A.srm1[t];
+    x0.x = ra * xt.x - rm * (x0.x - xt.x);
+    x0.y = ra * xt.y - rm * (x0.y - xt.y);
+    x0.z = ra * xt.z - rm * (x0.z - xt.z);
+  }
+  return x0;
+}
+
 // kFixed = false (no fixed set) compiles to the step as it was before fixed atoms existed.  kSeq = true runs step s of a respaced
 // chain (DESIGN.md section 1): the network saw t = seq_t[s], and the state moves to p = seq_p[s] with the per-step coefficients
-// seq_*[s]; kSeq = false is the default chain t = t_start - s, p = t - 1 on the checkpoint's tables.
+// seq_*[s]; kSeq = false is the default chain t = t_start - s, p = t - 1 on the checkpoint's tables.  A guided step (clash guidance)
+// runs these same instances with xm_final = the guided predictions and mean_noise = 0: the guidance kernel has already converted them.
 template <bool kFixed, bool kSeq>
 __global__ void step_epilogue_kernel(TdStepArgs A) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -185,13 +200,7 @@ __global__ void step_epilogue_kernel(TdStepArgs A) {
   // ---- positions: posterior mean + noise (reference :673-679)
   const int g = A.lig_graph[a];
   const float4 xt = A.lig_pos[a];
-  float4 x0 = A.xm_final[A.lig_node[a]];
-  if (A.mean_noise) {              // x0 = sqrt(1/ac) x_t - sqrt(1/ac - 1) (pred - x_t)   (reference :419-422,663-666)
-    const float ra = A.sra[t], rm = A.srm1[t];
-    x0.x = ra * xt.x - rm * (x0.x - xt.x);
-    x0.y = ra * xt.y - rm * (x0.y - xt.y);
-    x0.z = ra * xt.z - rm * (x0.z - xt.z);
-  }
+  const float4 x0 = td_pred_x0(A, a, t, xt);
   const float c0 = kSeq ? A.seq_c0[s] : A.c0[t], ct = kSeq ? A.seq_ct[s] : A.ct[t];
   const float sig = ((t == 0) ? 0.0f : 1.0f) * expf(0.5f * (kSeq ? A.seq_logvar[s] : A.logvar[t]));
   float4 xn;
@@ -267,6 +276,73 @@ void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st) {
     }
   }
   advance_step_kernel<<<1, 1, 0, st>>>(A.step);
+}
+
+// ---------------------------------------------------------------------------------------- clash guidance
+// Clash guidance (DESIGN.md section 1), before the epilogue of a denoising step: for ligand row a of graph g with the step's x0
+// prediction y (td_pred_x0), and each protein atom p of g at its bound position x_p, r = y - x_p, d = |r|; a pair contributes when
+// 0 < d < radius, and the guided prediction is y + strength * sum (radius - d) r / d over the contributing pairs, or y itself, bit for
+// bit, when none contributes.  It is written to row lig_node[a] of G.guided, a node-indexed array, which the unchanged epilogue then
+// reads as its xm_final.  One CTA per graph: the graph's protein coordinates pass through shared memory in chunks of
+// TD_GUIDE_CHUNK atoms; one warp per ligand atom, lane l summing the protein atoms j = l, l + 32, ... of the graph in order, then a
+// fixed shuffle tree.  The order of every sum depends on the graph's own atoms only, so a graph gets the same bits in any batch.
+#define TD_GUIDE_CHUNK 1024
+#define TD_GUIDE_WARPS 8
+__global__ void __launch_bounds__(TD_GUIDE_WARPS * 32) clash_guidance_kernel(TdStepArgs A, TdGuideArgs G) {
+  __shared__ float sx[TD_GUIDE_CHUNK], sy[TD_GUIDE_CHUNK], sz[TD_GUIDE_CHUNK];
+  const int g = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int p0 = G.node_ptr[g], np = G.prot_ptr[g + 1] - G.prot_ptr[g];       // protein nodes p0 .. p0 + np - 1 lead the graph
+  const int lb = G.node_ptr[g] - G.prot_ptr[g], le = G.node_ptr[g + 1] - G.prot_ptr[g + 1];
+  if (lb >= le) return;
+  const int s = *A.step;
+  const int t = A.seq_t ? A.seq_t[s] : A.t_start - s;
+  const float rho = G.radius, lam = G.strength;
+  const int nchunk = (np + TD_GUIDE_CHUNK - 1) / TD_GUIDE_CHUNK;
+  auto stage = [&](int c) {
+    __syncthreads();
+    for (int j = threadIdx.x; j < TD_GUIDE_CHUNK && c * TD_GUIDE_CHUNK + j < np; j += blockDim.x) {
+      const float4 x = G.prot_xm[p0 + c * TD_GUIDE_CHUNK + j];
+      sx[j] = x.x; sy[j] = x.y; sz[j] = x.z;
+    }
+    __syncthreads();
+  };
+  if (nchunk == 1) stage(0);
+  for (int base = lb; base < le; base += TD_GUIDE_WARPS) {      // every warp runs every round: the staging barriers are uniform
+    const int a = base + warp;
+    const bool live = a < le;
+    float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (live) y = td_pred_x0(A, a, t, A.lig_pos[a]);
+    float ax = 0.f, ay = 0.f, az = 0.f;
+    unsigned hit = 0;
+    for (int c = 0; c < nchunk; ++c) {
+      if (nchunk > 1) stage(c);
+      const int n = min(TD_GUIDE_CHUNK, np - c * TD_GUIDE_CHUNK);
+      if (!live) continue;
+      for (int j = lane; j < n; j += 32) {
+        const float rx = y.x - sx[j], ry = y.y - sy[j], rz = y.z - sz[j];
+        const float d = sqrtf(rx * rx + ry * ry + rz * rz);
+        if (d > 0.f && d < rho) {
+          const float w = (rho - d) / d;
+          ax += w * rx; ay += w * ry; az += w * rz;
+          hit = 1;
+        }
+      }
+    }
+    if (!live) continue;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      ax += __shfl_xor_sync(0xffffffffu, ax, o);
+      ay += __shfl_xor_sync(0xffffffffu, ay, o);
+      az += __shfl_xor_sync(0xffffffffu, az, o);
+    }
+    if (__any_sync(0xffffffffu, hit) && lane == 0) {
+      y.x = y.x + lam * ax; y.y = y.y + lam * ay; y.z = y.z + lam * az;
+    }
+    if (lane == 0) G.guided[A.lig_node[a]] = y;
+  }
+}
+void td_launch_clash_guidance(const TdStepArgs& A, const TdGuideArgs& G, int n_graphs, cudaStream_t st) {
+  if (A.n_lig > 0 && n_graphs > 0) clash_guidance_kernel<<<n_graphs, TD_GUIDE_WARPS * 32, 0, st>>>(A, G);
 }
 
 // Re-noising step s of a time path (tdiff_sample_path, DESIGN.md section 1): the state moves up from t = seq_t[s] to p = seq_p[s] > t

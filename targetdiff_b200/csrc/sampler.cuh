@@ -67,7 +67,16 @@ struct TdLikelihoodArgs {
   long long* vt;                   // [Nl] v_t, or NULL
 };
 
+// clash guidance (DESIGN.md section 1): the batch layout, the bound protein coordinates and the guided x0 predictions
+struct TdGuideArgs {
+  const int *node_ptr, *prot_ptr;  // [B+1]: graph g's protein atoms are nodes node_ptr[g] .. node_ptr[g] + prot_ptr[g+1] - prot_ptr[g] - 1
+  const float4* prot_xm;           // node array whose protein rows hold the bound, centred protein positions (xm0)
+  float4* guided;                  // out [N], node-indexed: row lig_node[a] <- the guided x0 prediction of ligand row a
+  float radius, strength;          // rho > 0 (A), lambda > 0
+};
+
 void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st);
+void td_launch_clash_guidance(const TdStepArgs& A, const TdGuideArgs& G, int n_graphs, cudaStream_t st);
 void td_launch_renoise(const TdStepArgs& A, cudaStream_t st);
 void td_launch_fixed_init(const TdStepArgs& A, cudaStream_t st);
 void td_launch_start_init(const TdStepArgs& A, cudaStream_t st);

@@ -17,7 +17,7 @@ import torch.nn.functional as F
 import torch.nn as nn
 
 from . import _lib
-from .config import Config, check_supported
+from .config import Config, check_clash_guidance, check_supported
 
 GAUSSIAN_OFFSETS = (0, 1, 1.25, 1.5, 1.75, 2, 2.25, 2.5, 2.75, 3, 3.5, 4, 4.5, 5, 5.5, 6, 7, 8, 9, 10)   # models/common.py:15
 
@@ -413,7 +413,7 @@ class ScorePosNet3D(nn.Module):
     def sample_diffusion(self, protein_pos, protein_v, batch_protein, init_ligand_pos, init_ligand_v, batch_ligand,
                          num_steps=None, center_pos_mode=None, pos_only=False, noise_tape=None, seed=None, return_traj=True,
                          stack_traj=False, fixed_mask=None, fixed_noise_tape=None, time_seq=None, start_time=None, start_noise_tape=None,
-                         time_path=None):
+                         time_path=None, clash_radius=None, clash_strength=0.0):
         """The reverse-diffusion chain (reference models/molopt_score_model.py:633-703), executed entirely by libtdiff.so.
 
         Extensions over the reference signature (all optional): `noise_tape=(pos_noise [S,Nl,3], v_uniform [S,Nl,K])`
@@ -443,8 +443,14 @@ class ScorePosNet3D(nn.Module):
         is time_seq's step, a re-noising step (p > tau_s) draws the state from the forward process q(x_p | x_t), q(v_p | v_t) without the
         network, and fixed rows are resampled at p after either.  Not with `time_seq`; it begins at the start time with `start_time`.
         Tapes are [S, ...] (fixed tape [S+1, ...]), trajectories [S, ...]; after a re-noising step v0_traj repeats the entry before and
-        vt_traj holds the normalised log q(v_p | v_t).  Sample quality is not measured."""
+        vt_traj holds the normalised log q(v_p | v_t).  Sample quality is not measured.
+
+        Clash guidance (DESIGN.md section 1): with `clash_strength` = lambda > 0 and `clash_radius` = rho, every denoising step moves
+        each ligand atom's x0 prediction y to y + lambda * sum (rho - d) (y - x_p) / d over the protein atoms x_p of its pocket at a
+        distance 0 < d < rho before the posterior step.  Every call sets the engine's guidance, off included, so a call never inherits
+        an earlier call's setting.  No random numbers are drawn.  Whether it improves molecules is not measured."""
         T = self.num_timesteps
+        clash_radius, clash_strength = check_clash_guidance(clash_radius, clash_strength)
         if time_path is not None:
             if time_seq is not None:
                 raise ValueError('time_path cannot be combined with time_seq')
@@ -476,6 +482,7 @@ class ScorePosNet3D(nn.Module):
         eng = self.engine(dev)
         lib = _lib.load()
         st = self._stream(dev)
+        _lib.check(lib.tdiff_set_clash_guidance(eng, ctypes.c_float(clash_radius or 0.0), ctypes.c_float(clash_strength)))
         B, Np, Nl = self._bind(eng, protein_pos, protein_v, batch_protein, batch_ligand, mode)
         lpos = init_ligand_pos.detach().to(torch.float32).contiguous()
         lv = init_ligand_v.detach().to(torch.int64).contiguous()
