@@ -234,6 +234,21 @@ TDIFF_API int tdiff_sample_path(tdiff_engine* e, const int32_t* h_time_path, int
  * belongs to the handle: it refers to no batch rows, so it survives tdiff_bind_batch.  Off on a new handle. */
 TDIFF_API int tdiff_set_clash_guidance(tdiff_engine* e, float radius, float strength);
 
+/* Element constraints (an extension beyond the reference, DESIGN.md section 1): d_allowed [Nl] uint32 (device), bit c of row a set =
+ * class c allowed for ligand atom a.  At every denoising step of every following chain (tdiff_sample, tdiff_sample_seq, the denoising
+ * steps of tdiff_sample_path, with or without clash guidance) the type head's log_softmax runs over the allowed classes only (the
+ * others get log v0_hat = -inf: the prediction conditioned on v0 in the set), and the posterior runs unchanged on it.  On the decoder
+ * step (target time p < 0: t = 0 of the default chain, or a sequence or path ending at 0) the posterior is also renormalised over the
+ * allowed set, so that the draw picks an allowed class.  The intermediate states are drawn from the whole posterior (the forward
+ * marginals have mass on every class), so a chain that stops before t = 0 may end in a forbidden class.  v0_traj holds the conditioned
+ * log v0_hat and vt_traj the distribution each state was drawn from, -inf at forbidden entries where that is their value.  A mask
+ * that allows every class gives the unconstrained chain's bits.  No random numbers are drawn; no launch is added per step.  Fixed rows
+ * (tdiff_set_fixed) are overwritten as before.  Re-noising steps, the start and fixed-row draws, tdiff_forward, tdiff_forward_blocks
+ * and tdiff_likelihood_terms ignore the mask.  NULL clears it.  A row without a class or with a bit at or above num_classes ->
+ * TDIFF_EINVAL and the previous mask stays (synchronises the stream).  A chain with pos_only while a mask is set -> TDIFF_EINVAL.
+ * Before tdiff_bind_batch -> TDIFF_ESTATE; tdiff_bind_batch clears the mask. */
+TDIFF_API int tdiff_set_type_mask(tdiff_engine* e, const uint32_t* d_allowed, void* stream);
+
 /* Start-ligand sampling (an extension beyond the reference, DESIGN.md section 1): arms the next chains to start from the current ligand
  * state (the start ligand x0, v0, centred like any ligand) noised to the start time t_start in 0..T-1, and to run the reverse chain
  * from there; t_start = -1 clears it.  The current ligand state is the one tdiff_set_ligand set or, after a chain, that chain's

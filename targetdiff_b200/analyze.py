@@ -66,3 +66,22 @@ def protein_contacts(ligand_pos, protein_pos, batch_ligand, batch_protein, radiu
         n_close[g] = int((d < radius).sum())
         d_min[g] = float(d.min())
     return n_close, d_min
+
+
+def type_violations(v, allowed):
+    """Atoms whose class is outside the allowed set.  v: class indices [n] (array or tensor, or a list of per-molecule arrays);
+    allowed: class indices, a [K] bool mask, or a per-atom [n,K] bool mask.  Returns the count as an int (element constraints,
+    DESIGN.md section 1)."""
+    if isinstance(v, (list, tuple)):
+        v = np.concatenate([np.asarray(x).reshape(-1) for x in v]) if len(v) else np.zeros(0, np.int64)
+    v = torch.as_tensor(np.asarray(v)).long().reshape(-1)
+    a = torch.as_tensor(np.asarray(allowed.cpu() if torch.is_tensor(allowed) else allowed))
+    if a.dtype == torch.bool and a.dim() == 2:
+        if a.shape[0] != len(v):
+            raise ValueError('a per-atom mask needs one row per atom: %d rows, %d atoms' % (a.shape[0], len(v)))
+        ok = a[torch.arange(len(v)), v]
+    elif a.dtype == torch.bool:
+        ok = a[v]
+    else:
+        ok = torch.isin(v, a.long().reshape(-1))
+    return int((~ok).sum())

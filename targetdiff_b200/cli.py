@@ -30,7 +30,10 @@ run the n-step chain of sampling.respaced_time_seq(T, n) instead of num_steps, a
 `sample.resamplings: r` > 1 (and `sample.jump_length: j`, default 1) sample_for_pocket runs sampling.resampled_time_path over that
 chain, with a --fragment or kept atoms only, and sample.pt also holds 'time_path'; sample_pockets refuses the key.  With
 `sample.clash_strength: lambda` > 0 and `sample.clash_radius: rho` (config.sample_clash_guidance; strength 0, the default, is off) both
-commands run clash guidance (ScorePosNet3D.sample_diffusion), and the result also holds 'clash_guidance': {'radius', 'strength'}.  Molecule
+commands run clash guidance (ScorePosNet3D.sample_diffusion), and the result also holds 'clash_guidance': {'radius', 'strength'}.  With
+`sample.allowed_elements: [C, N, O, ...]` or `sample.allowed_classes: [...]` (config.sample_allowed_classes, in the checkpoint's
+ligand_atom_mode) both commands constrain every free atom of the finished molecules to those classes, and the result also holds
+'allowed_classes'.  Molecule
 reconstruction / SDF writing needs RDKit + OpenBabel and stays out of scope."""
 import argparse
 import os
@@ -39,21 +42,36 @@ import sys
 
 import torch
 
-from .config import check_resampling, load_config, sample_clash_guidance, sampling_start, sampling_time_path, sampling_time_seq
+from .config import (check_resampling, load_config, sample_allowed_classes, sample_clash_guidance, sampling_start, sampling_time_path,
+                     sampling_time_seq)
 from .likelihood import likelihood_time_steps, ligand_nll
-from .pocket import pdb_to_pocket_data
+from .pocket import LIGAND_CLASS_ELEMENTS, pdb_to_pocket_data
 from .sampling import sample_diffusion_ligand, seed_all
 from .score_model import ScorePosNet3D
 
 
 PROTEIN_FEATURE_DIM = 27                                                    # reference utils/transforms.py:115-132
-LIGAND_ATOM_MODE_CLASSES = {'basic': 8, 'add_aromatic': 13, 'full': 23}     # len(MAP_ATOM_TYPE_*_TO_INDEX), utils/transforms.py:11-66,143-149
+LIGAND_ATOM_MODE_CLASSES = {m: len(z) for m, z in LIGAND_CLASS_ELEMENTS.items()}   # len(MAP_ATOM_TYPE_*_TO_INDEX), utils/transforms.py:11-66,143-149
 
 
 def build_result(data, outputs):
     pred_pos, pred_v, pred_pos_traj, pred_v_traj, pred_v0_traj, pred_vt_traj, time_list = outputs
     return {'data': data, 'pred_ligand_pos': pred_pos, 'pred_ligand_v': pred_v, 'pred_ligand_pos_traj': pred_pos_traj,
             'pred_ligand_v_traj': pred_v_traj, 'time': time_list}
+
+
+def _allowed_classes(config, model):
+    """The element constraint of the config (config.sample_allowed_classes) in the checkpoint's ligand atom mode, or None."""
+    if config.sample.get('allowed_elements') is None and config.sample.get('allowed_classes') is None:
+        return None
+    return sample_allowed_classes(config.sample, model.ligand_atom_mode)
+
+
+def add_allowed_classes(result, allowed):
+    """Record an element constraint in a result dict; nothing without one, so the file is as without it."""
+    if allowed is not None:
+        result['allowed_classes'] = list(allowed)
+    return result
 
 
 def add_clash_guidance(result, radius, strength):
@@ -79,6 +97,7 @@ def _load_model(config, device, rank=0):
     if mode not in LIGAND_ATOM_MODE_CLASSES:
         raise NotImplementedError('checkpoint ligand_atom_mode=%r (known: %s)' % (mode, sorted(LIGAND_ATOM_MODE_CLASSES)))
     model = ScorePosNet3D(get(tc, 'model'), PROTEIN_FEATURE_DIM, LIGAND_ATOM_MODE_CLASSES[mode])
+    model.ligand_atom_mode = mode
     if rank == 0:
         model.load_state_dict(ckpt['model'])
     model = model.to(device)
@@ -151,6 +170,7 @@ def sample_pockets(argv):
     paths = list_pockets(a.pocket_dir, a.pocket_list)
     mine = assign_pockets(paths, rank, world, a.schedule, a.data_id)
     model = _load_model(config, device, rank)
+    allowed = _allowed_classes(config, model)
     time_seq = _time_seq(config, model)
     num_steps = config.sample.num_steps if time_seq is None else None
     n = a.num_samples if a.num_samples is not None else config.sample.num_samples
@@ -164,8 +184,8 @@ def sample_pockets(argv):
         outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=device, num_steps=num_steps,
                                           pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
                                           sample_num_atoms=config.sample.sample_num_atoms, time_seq=time_seq,
-                                          clash_radius=clash_radius, clash_strength=clash_strength)
-        result = add_clash_guidance(build_result(data, outputs), clash_radius, clash_strength)
+                                          clash_radius=clash_radius, clash_strength=clash_strength, allowed_types=allowed)
+        result = add_allowed_classes(add_clash_guidance(build_result(data, outputs), clash_radius, clash_strength), allowed)
         if time_seq is not None:
             result['time_seq'] = time_seq
         torch.save(result, os.path.join(a.result_path, 'result_%d.pt' % i))
@@ -236,6 +256,7 @@ def sample_for_pocket(argv):
     clash_radius, clash_strength = sample_clash_guidance(config.sample)
     seed_all(config.sample.seed)
     model = _load_model(config, a.device)
+    allowed = _allowed_classes(config, model)
     start_time, start_seq = sampling_start(config.sample, model.num_timesteps, start is not None)
     time_seq = _time_seq(config, model) if start is None else start_seq
     T = model.num_timesteps
@@ -251,10 +272,10 @@ def sample_for_pocket(argv):
                                       pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
                                       sample_num_atoms=config.sample.sample_num_atoms, fixed_ligand=fragment,
                                       time_seq=time_seq if time_path is None else None, clash_radius=clash_radius,
-                                      clash_strength=clash_strength, **kw)
+                                      clash_strength=clash_strength, allowed_types=allowed, **kw)
     os.makedirs(a.result_path, exist_ok=True)
     shutil.copyfile(a.config, os.path.join(a.result_path, 'sample.yml'))
-    result = add_clash_guidance(build_result(data, outputs), clash_radius, clash_strength)
+    result = add_allowed_classes(add_clash_guidance(build_result(data, outputs), clash_radius, clash_strength), allowed)
     if fragment is not None:
         result['fixed_ligand_atoms'] = int(fragment[1].shape[0])
     if start is not None:

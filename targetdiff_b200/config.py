@@ -128,6 +128,30 @@ def sample_clash_guidance(sample):
     return check_clash_guidance(sample.get('clash_radius'), sample.get('clash_strength', 0.0))
 
 
+def sample_allowed_classes(sample, mode):
+    """Sorted class indices of the ligand atom mode `mode` that the element constraint of `sample.allowed_elements` (element symbols,
+    e.g. [C, N, O]: every class of those elements) or `sample.allowed_classes` (class indices) allows, or None without either (an
+    extension beyond the reference's sampling.yml, DESIGN.md section 1).  ValueError when both are given, for an empty list, an
+    unknown symbol (the message lists the mode's elements) or a class outside 0..K-1."""
+    from .pocket import LIGAND_CLASS_ELEMENTS, element_classes
+    el, cl = sample.get('allowed_elements'), sample.get('allowed_classes')
+    if el is not None and cl is not None:
+        raise ValueError('give sample.allowed_elements or sample.allowed_classes, not both')
+    if el is None and cl is None:
+        return None
+    if el is not None:
+        if isinstance(el, str) or not isinstance(el, (list, tuple)):
+            raise ValueError('sample.allowed_elements must be a list of element symbols, got %r' % (el,))
+        return element_classes(el, mode)
+    K = len(LIGAND_CLASS_ELEMENTS[mode])
+    if not isinstance(cl, (list, tuple)) or not cl:
+        raise ValueError('sample.allowed_classes must be a non-empty list of class indices, got %r' % (cl,))
+    for c in cl:
+        if isinstance(c, bool) or not isinstance(c, int) or not 0 <= c < K:
+            raise ValueError('sample.allowed_classes: %r is not a class index of the %s mode (0..%d)' % (c, mode, K - 1))
+    return sorted(set(cl))
+
+
 def sampling_time_path(sample, T, base, held):
     """The resampled time path of check_resampling's (r, j): sampling.resampled_time_path over `base`, the chain's decreasing time
     sequence (T - 1, ..., 0 when it is None), or None when r = 1."""

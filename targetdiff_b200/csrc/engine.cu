@@ -148,6 +148,9 @@ struct tdiff_engine {
   // [N] float4: the guided x0 predictions of a step at the ligand rows (clash_guidance_kernel), the epilogue's xm_final
   float clash_radius = 0.f, clash_strength = 0.f;
   DevBuf guided;
+  // element constraints (tdiff_set_type_mask): [Nl] uint32 class bit masks, armed while has_type_mask; cleared by tdiff_bind_batch
+  bool has_type_mask = false;
+  DevBuf type_mask;
   DevBuf stage[8];   // staging for tdiff_sample_host
   // ---- instrumentation
   cudaStream_t own_stream = nullptr;   // capture stream (the caller's stream may be the legacy default stream, which cannot capture)
@@ -637,7 +640,7 @@ extern "C" void tdiff_destroy(tdiff_engine* e) {
   if (e->ev_join) cudaEventDestroy(e->ev_join);
   DevBuf* bufs[] = {&e->node_ptr, &e->prot_ptr, &e->prot_node, &e->prot_graph, &e->lig_node, &e->lig_graph, &e->node_lig, &e->xm0, &e->xm1,
                     &e->rel_flag, &e->rel_list, &e->n_rel, &e->work_list, &e->n_work, &e->knn_cache, &e->x2h_rows, &e->lig_rows, &e->cone_rows, &e->cone_counts, &e->ew_x2h, &e->ew_h2x, &e->h_sync, &e->hagg, &e->time_norm, &e->h_free, &e->dirty, &e->free_rows, &e->free_counts, &e->lig_save, &e->offset, &e->h0, &e->h, &e->P, &e->q, &e->src, &e->src_prev, &e->etype, &e->e_w, &e->dist, &e->kbuf, &e->vbuf, &e->v16, &e->lig_pos,
-                    &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges, &e->fix_mask, &e->fix_pos, &e->fix_v, &e->seq_buf, &e->lk_buf, &e->lk_x0, &e->lk_v0};
+                    &e->lig_v, &e->logits, &e->step, &e->err_flag, &e->node_off, &e->total_edges, &e->fix_mask, &e->fix_pos, &e->fix_v, &e->seq_buf, &e->lk_buf, &e->lk_x0, &e->lk_v0, &e->type_mask};
   for (auto* b : bufs) b->release();
   for (auto& b : e->stage) b.release();
   if (e->arena) cudaFree(e->arena);
@@ -690,7 +693,7 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   }
   node_ptr[B] = n; prot_ptr[B] = p;
   e->bound = false; e->has_ligand = false; e->have_graph = false; e->have_prev = false; e->cone_evals = 0;
-  e->has_fixed = false; e->fix_pos_noise = nullptr; e->fix_v_uniform = nullptr;
+  e->has_fixed = false; e->fix_pos_noise = nullptr; e->fix_v_uniform = nullptr; e->has_type_mask = false;
   e->start_t = -1; e->start_pos_noise = nullptr; e->start_v_uniform = nullptr;
   e->B = B; e->N = (int)N; e->Np = (int)Np; e->Nl = (int)Nl; e->max_ng = max_ng;
   const size_t slots = (size_t)N * K;
@@ -1248,7 +1251,7 @@ void run_step(tdiff_engine* e, cudaStream_t st, const TdStepArgs& base) {
     A.mean_noise = 0;
     e->launches += 1;
   }
-  td_launch_step_epilogue(A, st);
+  td_launch_step_epilogue(A, e->has_type_mask ? e->type_mask.as<uint32_t>() : nullptr, st);
   e->launches += 2;
 }
 // Per-step tables of the respaced chain `seq` [S] (DESIGN.md section 1), laid out as e->seq_buf: seq_t, seq_p [S] int32, then c0, ct,
@@ -1340,6 +1343,8 @@ int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const 
   }
   if ((d_pos_noise == nullptr) != (d_v_uniform == nullptr) && !pos_only)
     return set_err(TDIFF_EINVAL, "noise tape needs both pos_noise and v_uniform (or neither for Philox)");
+  if (pos_only && e->has_type_mask)
+    return set_err(TDIFF_EINVAL, "a type mask is set (tdiff_set_type_mask) but pos_only keeps every atom type: clear the mask, or sample types");
   if (e->has_fixed) {      // one noise source per chain: both tapes or neither
     if ((d_pos_noise != nullptr) != (e->fix_pos_noise != nullptr))
       return set_err(TDIFF_EINVAL, d_pos_noise ? "fixed atoms with a noise tape need a fixed-atom tape (tdiff_set_fixed_tape)"
@@ -1486,6 +1491,38 @@ extern "C" int tdiff_set_clash_guidance(tdiff_engine* e, float radius, float str
     return set_err(TDIFF_EINVAL, "set_clash_guidance: radius=%g must be finite and > 0 when strength > 0", (double)radius);
   e->clash_strength = strength;
   e->clash_radius = strength > 0.f ? radius : 0.f;
+  return TDIFF_OK;
+}
+
+// Element constraints (DESIGN.md section 1): the mask is checked on the device before it replaces the armed one, so that a refused
+// call leaves the previous mask in place.
+extern "C" int tdiff_set_type_mask(tdiff_engine* e, const uint32_t* d_allowed, void* stream) {
+  if (!e || !e->bound) return set_err(TDIFF_ESTATE, "set_type_mask before bind_batch");
+  if (!d_allowed) {
+    e->has_type_mask = false;
+    return TDIFF_OK;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  CK(cudaSetDevice(e->device));
+  const size_t Nl = (size_t)e->Nl;
+  const int K = e->cfg.num_classes;
+  td_launch_check_type_mask(d_allowed, e->Nl, K, e->err_flag.as<int>(), st);
+  e->launches += 1;
+  int flag = 0;
+  CK(cudaMemcpyAsync(&flag, e->err_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (flag) {
+    cudaMemsetAsync(e->err_flag.p, 0, sizeof(int), st);
+    return set_err(TDIFF_EINVAL, "set_type_mask: a row allows no class, or a bit at or above num_classes (%d) is set", K);
+  }
+  // an armed mask belongs to the bound batch, whose Nl rows the buffer already holds: ensure never reallocates under it
+  if (e->type_mask.ensure(Nl * 4 + 16)) {
+    e->has_type_mask = false;
+    return set_err(TDIFF_ECUDA, "out of device memory for the type mask of %zu ligand atoms", Nl);
+  }
+  if (Nl) CK(cudaMemcpyAsync(e->type_mask.p, d_allowed, Nl * 4, cudaMemcpyDeviceToDevice, st));
+  CK(cudaGetLastError());
+  e->has_type_mask = true;
   return TDIFF_OK;
 }
 

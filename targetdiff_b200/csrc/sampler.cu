@@ -157,8 +157,12 @@ __device__ __forceinline__ float4 td_pred_x0(const TdStepArgs& A, int a, int t, 
 // chain (DESIGN.md section 1): the network saw t = seq_t[s], and the state moves to p = seq_p[s] with the per-step coefficients
 // seq_*[s]; kSeq = false is the default chain t = t_start - s, p = t - 1 on the checkpoint's tables.  A guided step (clash guidance)
 // runs these same instances with xm_final = the guided predictions and mean_noise = 0: the guidance kernel has already converted them.
-template <bool kFixed, bool kSeq>
-__global__ void step_epilogue_kernel(TdStepArgs A) {
+// kMask = true (element constraints, DESIGN.md section 1): bit c of allowed[a] set = class c allowed for row a.  The type head's
+// log_softmax runs over the allowed classes only (the others enter as -inf, so exp gives exactly 0 and every sum is unchanged when all
+// are allowed), and on the decoder step (p < 0) the posterior's forbidden classes are -inf before its normalisation, so that it is
+// renormalised over the allowed set and the Gumbel-max draw can only pick an allowed class.  kMask = false never reads `allowed`.
+template <bool kFixed, bool kSeq, bool kMask>
+__global__ void step_epilogue_kernel(TdStepArgs A, const uint32_t* __restrict__ allowed) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a >= A.n_lig) return;
   const int s = *A.step;                       // steps done so far
@@ -224,7 +228,11 @@ __global__ void step_epilogue_kernel(TdStepArgs A) {
     const float* lg = A.logits + (size_t)a * K;
     float lr[TD_CMAX];
     float mx = -INFINITY;
-    for (int c = 0; c < K; ++c) { lr[c] = lg[c]; mx = fmaxf(mx, lr[c]); }
+    const uint32_t am = kMask ? allowed[a] : 0u;
+    for (int c = 0; c < K; ++c) {
+      lr[c] = (kMask && !((am >> c) & 1u)) ? -INFINITY : lg[c];
+      mx = fmaxf(mx, lr[c]);
+    }
     float se = 0.0f;
     for (int c = 0; c < K; ++c) se += expf(lr[c] - mx);
     const float lse = logf(se);
@@ -239,6 +247,7 @@ __global__ void step_epilogue_kernel(TdStepArgs A) {
     for (int c = 0; c < K; ++c) {
       const float lvt = (c == vcur) ? 0.0f : log_eps;
       un_lp[c] = log_add_exp_f(lr[c] + lca, l1mca) + log_add_exp_f(lvt + la, l1ma);
+      if (kMask && p < 0 && !((am >> c) & 1u)) un_lp[c] = -INFINITY;       // decoder step: renormalised over the allowed set
       m2 = fmaxf(m2, un_lp[c]);
     }
     float s2 = 0.0f;
@@ -264,16 +273,21 @@ __global__ void step_epilogue_kernel(TdStepArgs A) {
 
 __global__ void advance_step_kernel(int* step) { *step += 1; }
 
-void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st) {
+template <bool kMask>
+static void launch_step_epilogue(const TdStepArgs& A, const uint32_t* allowed, int grid, cudaStream_t st) {
+  if (A.seq_t) {
+    if (A.fix_mask) step_epilogue_kernel<true, true, kMask><<<grid, 128, 0, st>>>(A, allowed);
+    else step_epilogue_kernel<false, true, kMask><<<grid, 128, 0, st>>>(A, allowed);
+  } else {
+    if (A.fix_mask) step_epilogue_kernel<true, false, kMask><<<grid, 128, 0, st>>>(A, allowed);
+    else step_epilogue_kernel<false, false, kMask><<<grid, 128, 0, st>>>(A, allowed);
+  }
+}
+void td_launch_step_epilogue(const TdStepArgs& A, const uint32_t* allowed, cudaStream_t st) {
   if (A.n_lig > 0) {
     const int grid = (A.n_lig + 127) / 128;
-    if (A.seq_t) {
-      if (A.fix_mask) step_epilogue_kernel<true, true><<<grid, 128, 0, st>>>(A);
-      else step_epilogue_kernel<false, true><<<grid, 128, 0, st>>>(A);
-    } else {
-      if (A.fix_mask) step_epilogue_kernel<true, false><<<grid, 128, 0, st>>>(A);
-      else step_epilogue_kernel<false, false><<<grid, 128, 0, st>>>(A);
-    }
+    if (allowed) launch_step_epilogue<true>(A, allowed, grid, st);
+    else launch_step_epilogue<false>(A, nullptr, grid, st);
   }
   advance_step_kernel<<<1, 1, 0, st>>>(A.step);
 }
@@ -628,6 +642,18 @@ void td_launch_set_fixed(const unsigned char* mask, const float* pos, const long
                          cudaStream_t st) {
   if (n > 0) set_fixed_kernel<<<(n + 255) / 256, 256, 0, st>>>(mask, pos, v, lig_graph, offset, apply_center, n, n_classes, fix_mask, fix_pos,
                                                                fix_v, err);
+}
+
+// type mask in (tdiff_set_type_mask): every row needs a class and no bit at or above n_classes; only checked, the caller copies
+__global__ void check_type_mask_kernel(const uint32_t* __restrict__ allowed, int n, int n_classes, int* __restrict__ err) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= n) return;
+  const uint32_t m = allowed[a];
+  const uint32_t outside = n_classes >= 32 ? 0u : ~((1u << n_classes) - 1u);
+  if (m == 0u || (m & outside)) atomicExch(err, 1);
+}
+void td_launch_check_type_mask(const uint32_t* allowed, int n, int n_classes, int* err, cudaStream_t st) {
+  if (n > 0) check_type_mask_kernel<<<(n + 255) / 256, 256, 0, st>>>(allowed, n, n_classes, err);
 }
 
 // ---------------------------------------------------------------------------------------- state marshalling

@@ -75,7 +75,9 @@ struct TdGuideArgs {
   float radius, strength;          // rho > 0 (A), lambda > 0
 };
 
-void td_launch_step_epilogue(const TdStepArgs& A, cudaStream_t st);
+// allowed: [Nl] class bit masks of the element constraint (tdiff_set_type_mask), or NULL for the unconstrained step
+void td_launch_step_epilogue(const TdStepArgs& A, const uint32_t* allowed, cudaStream_t st);
+void td_launch_check_type_mask(const uint32_t* allowed, int n, int n_classes, int* err, cudaStream_t st);
 void td_launch_clash_guidance(const TdStepArgs& A, const TdGuideArgs& G, int n_graphs, cudaStream_t st);
 void td_launch_renoise(const TdStepArgs& A, cudaStream_t st);
 void td_launch_fixed_init(const TdStepArgs& A, cudaStream_t st);

@@ -83,6 +83,40 @@ def pdb_to_pocket_data(pdb_path_or_block):
 # index -> (atomic number, aromatic) of the 13 ligand classes, 'add_aromatic' mode (utils/transforms.py:48-62,69-90)
 LIGAND_CLASS_TO_ATOM = ((1, False), (6, False), (6, True), (7, False), (7, True), (8, False), (8, True), (9, False), (15, False), (15, True),
                         (16, False), (16, True), (17, False))
+# index -> atomic number of the 8 ligand classes, 'basic' mode (utils/transforms.py:37-46)
+LIGAND_CLASS_TO_ATOM_BASIC = (1, 6, 7, 8, 9, 15, 16, 17)
+# index -> (atomic number, hybridization, aromatic) of the 23 ligand classes, 'full' mode (utils/transforms.py:11-35)
+LIGAND_CLASS_TO_ATOM_FULL = ((1, 'S', False), (6, 'SP', False), (6, 'SP2', False), (6, 'SP2', True), (6, 'SP3', False), (7, 'SP', False),
+                             (7, 'SP2', False), (7, 'SP2', True), (7, 'SP3', False), (8, 'SP2', False), (8, 'SP2', True), (8, 'SP3', False),
+                             (9, 'SP3', False), (15, 'SP2', False), (15, 'SP2', True), (15, 'SP3', False), (15, 'SP3D', False),
+                             (16, 'SP2', False), (16, 'SP2', True), (16, 'SP3', False), (16, 'SP3D', False), (16, 'SP3D2', False),
+                             (17, 'SP3', False))
+# ligand_atom_mode -> the atomic number of each class
+LIGAND_CLASS_ELEMENTS = {'basic': LIGAND_CLASS_TO_ATOM_BASIC, 'add_aromatic': tuple(z for z, _ in LIGAND_CLASS_TO_ATOM),
+                         'full': tuple(z for z, _, _ in LIGAND_CLASS_TO_ATOM_FULL)}
+ELEMENT_SYMBOL = {z: sym for sym, z in ATOMIC_NUMBER.items() if sym != 'D'}
+
+
+def element_classes(symbols, mode='add_aromatic'):
+    """Sorted class indices of `mode` whose element is one of `symbols` (e.g. ['C', 'N', 'O']): every class of an element, so that
+    in 'add_aromatic' 'C' gives the aliphatic and the aromatic carbon, and in 'full' every hybridization.  ValueError for an unknown
+    mode, an empty list, or a symbol that no class of the mode has (the message lists the mode's elements)."""
+    if mode not in LIGAND_CLASS_ELEMENTS:
+        raise ValueError('ligand_atom_mode %r (known: %s)' % (mode, sorted(LIGAND_CLASS_ELEMENTS)))
+    zs = LIGAND_CLASS_ELEMENTS[mode]
+    known = [ELEMENT_SYMBOL[z] for z in sorted(set(zs))]
+    if isinstance(symbols, str):
+        symbols = [symbols]
+    symbols = list(symbols)
+    if not symbols:
+        raise ValueError('an element constraint needs at least one element (%s mode: %s)' % (mode, ', '.join(known)))
+    want = set()
+    for sym in symbols:
+        z = ATOMIC_NUMBER.get(str(sym).strip().capitalize()) if isinstance(sym, str) else None
+        if z not in zs:
+            raise ValueError('element %r is not a ligand class of the %s mode (its elements: %s)' % (sym, mode, ', '.join(known)))
+        want.add(z)
+    return [c for c, z in enumerate(zs) if z in want]
 
 
 def get_atomic_number_from_index(index, mode='add_aromatic'):

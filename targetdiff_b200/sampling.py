@@ -38,7 +38,15 @@ Resampled sampling (an extension beyond the reference, DESIGN.md section 1; RePa
 state back up with the forward process, so that the free atoms are denoised again next to the held fragment or kept atoms
 (ScorePosNet3D.sample_diffusion(time_path=...)).  Not with `time_seq`; with a start ligand the path begins at the start time.  Under
 rng='cpu' the draws are those of a time_seq of S = len(time_path) steps.  Whether resampling improves the molecules has not been
-measured."""
+measured.
+
+Element constraints (an extension beyond the reference, DESIGN.md section 1).  `allowed_types` restricts the classes the free atoms
+end in: class indices or a [K] bool for every free atom (pocket.element_classes maps element symbols to a mode's classes), or with a
+start ligand a [n, K] bool with one row per start atom (e.g. "this position must be N or O").  Fragment and kept atoms get every class.
+Each denoising step conditions the type prediction on the set and the decoder step draws from the posterior renormalised over it
+(ScorePosNet3D.sample_diffusion(allowed_types=...)), so a chain that ends at t = 0 uses only allowed classes; a set of every class
+runs the plain chain.  No random numbers are drawn, so the rng='cpu' order is unchanged.  Not with pos_only.  Whether constrained
+molecules are chemically sensible has not been measured."""
 import time
 
 import numpy as np
@@ -142,17 +150,53 @@ def _check_start(model,start_ligand, start_time, keep_atoms, fixed_ligand):
     return pos, v, t0, keep
 
 
+def _check_allowed(allowed_types, K, start, pos_only):
+    """The element constraint of sample_diffusion_ligand as a [K] bool (every free atom) or [n, K] bool (each start atom), or None
+    without one; ValueError for what sample_diffusion_ligand refuses."""
+    if allowed_types is None:
+        return None
+    if pos_only:
+        raise ValueError('allowed_types constrains atom types, which pos_only=True keeps as they are')
+    a = torch.as_tensor(allowed_types).detach().cpu()
+    if a.numel() == 0:
+        raise ValueError('allowed_types is empty: every atom needs at least one allowed class')
+    if a.dtype == torch.bool and a.dim() == 2:
+        if start is None:
+            raise ValueError('a per-atom allowed_types [n, K] needs a start_ligand: its rows are the start atoms')
+        if tuple(a.shape) != (len(start[1]), K):
+            raise ValueError('a per-atom allowed_types must be [n, K] = %s, got %s' % ((len(start[1]), K), tuple(a.shape)))
+        m = a
+    elif a.dtype == torch.bool:
+        if a.dim() != 1 or len(a) != K:
+            raise ValueError('a bool allowed_types must be [K] = [%d] or, with a start_ligand, [n, K]; got %s' % (K, tuple(a.shape)))
+        m = a
+    else:
+        if a.is_floating_point() or a.is_complex() or a.dim() > 1:
+            raise ValueError('allowed_types must be class indices, a [K] bool or a per-atom [n, K] bool; got %s %s' % (tuple(a.shape), a.dtype))
+        idx = a.reshape(-1).long()
+        if int(idx.min()) < 0 or int(idx.max()) >= K:
+            raise ValueError('allowed_types classes must lie in 0..%d' % (K - 1))
+        m = torch.zeros(K, dtype=torch.bool)
+        m[idx] = True
+    empty = (~m.reshape(-1, K).any(1)).nonzero().reshape(-1).tolist()
+    if empty:
+        raise ValueError('allowed_types allows no class for %s' % ('any atom' if m.dim() == 1 else 'start atom(s) %s' % empty))
+    return m
+
+
 def _split(arr, cum, n_data):
     return [arr[..., cum[k]:cum[k + 1], :] if arr.ndim == 3 else arr[..., cum[k]:cum[k + 1]] for k in range(n_data)]
 
 
 def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cuda:0', num_steps=None, pos_only=False,
                             center_pos_mode='protein', sample_num_atoms='prior', rng='device', fixed_ligand=None, time_seq=None,
-                            start_ligand=None, start_time=None, keep_atoms=None, time_path=None, clash_radius=None, clash_strength=0.0):
+                            start_ligand=None, start_time=None, keep_atoms=None, time_path=None, clash_radius=None, clash_strength=0.0,
+                            allowed_types=None):
     if rng not in ('device', 'cpu'):
         raise ValueError("rng must be 'device' or 'cpu'")
     clash_radius, clash_strength = check_clash_guidance(clash_radius, clash_strength)     # draws nothing: rng='cpu' order unchanged
     start = _check_start(model, start_ligand, start_time, keep_atoms, fixed_ligand)
+    allowed = _check_allowed(allowed_types, model.num_classes, start, pos_only)          # draws nothing either
     if time_path is not None:
         if time_seq is not None:
             raise ValueError('time_path cannot be combined with time_seq')
@@ -265,6 +309,13 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
                 extra['fixed_mask'] = mask
                 if rng == 'cpu':
                     extra['fixed_noise_tape'] = (torch.randn(S + 1, n_lig, 3), torch.rand(S + 1, n_lig, model.num_classes))
+            if allowed is not None:                                     # fragment and kept rows: every class
+                am = allowed.expand(n_lig, -1).clone() if allowed.dim() == 1 else allowed.repeat(n_data, 1)
+                am = am.to(device)
+                if 'fixed_mask' in extra:
+                    am[extra['fixed_mask']] = True
+                if not bool(am.all()):
+                    extra['allowed_types'] = am
 
             r = model.sample_diffusion(protein_pos=protein_pos, protein_v=protein_v, batch_protein=batch_protein,
                                        init_ligand_pos=init_ligand_pos, init_ligand_v=init_ligand_v, batch_ligand=batch_ligand,

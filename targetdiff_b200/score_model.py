@@ -413,7 +413,7 @@ class ScorePosNet3D(nn.Module):
     def sample_diffusion(self, protein_pos, protein_v, batch_protein, init_ligand_pos, init_ligand_v, batch_ligand,
                          num_steps=None, center_pos_mode=None, pos_only=False, noise_tape=None, seed=None, return_traj=True,
                          stack_traj=False, fixed_mask=None, fixed_noise_tape=None, time_seq=None, start_time=None, start_noise_tape=None,
-                         time_path=None, clash_radius=None, clash_strength=0.0):
+                         time_path=None, clash_radius=None, clash_strength=0.0, allowed_types=None):
         """The reverse-diffusion chain (reference models/molopt_score_model.py:633-703), executed entirely by libtdiff.so.
 
         Extensions over the reference signature (all optional): `noise_tape=(pos_noise [S,Nl,3], v_uniform [S,Nl,K])`
@@ -448,9 +448,19 @@ class ScorePosNet3D(nn.Module):
         Clash guidance (DESIGN.md section 1): with `clash_strength` = lambda > 0 and `clash_radius` = rho, every denoising step moves
         each ligand atom's x0 prediction y to y + lambda * sum (rho - d) (y - x_p) / d over the protein atoms x_p of its pocket at a
         distance 0 < d < rho before the posterior step.  Every call sets the engine's guidance, off included, so a call never inherits
-        an earlier call's setting.  No random numbers are drawn.  Whether it improves molecules is not measured."""
+        an earlier call's setting.  No random numbers are drawn.  Whether it improves molecules is not measured.
+
+        Element constraints (DESIGN.md section 1): `allowed_types` [Nl, K] bool, row a the classes ligand atom a may end in (none
+        empty).  Every denoising step conditions the type prediction on the allowed set (log v0_hat = -inf elsewhere) and the decoder
+        step (the last step of a chain that ends at t = 0) draws from the posterior renormalised over it, so every atom of a chain
+        that ends at t = 0 ends in an allowed class; intermediate states, and the last state of a chain that stops before t = 0, are
+        not restricted.  Fixed rows are held as without it (give them every class).  v0_traj / vt_traj hold -inf at forbidden
+        entries where those are their values.  Not with pos_only.  Every call sets or clears the engine's mask.  No random numbers
+        are drawn.  Whether constrained molecules are chemically sensible is not measured."""
         T = self.num_timesteps
         clash_radius, clash_strength = check_clash_guidance(clash_radius, clash_strength)
+        if allowed_types is not None and pos_only:
+            raise ValueError('allowed_types constrains atom types, which pos_only=True keeps as they are')
         if time_path is not None:
             if time_seq is not None:
                 raise ValueError('time_path cannot be combined with time_seq')
@@ -488,6 +498,13 @@ class ScorePosNet3D(nn.Module):
         lv = init_ligand_v.detach().to(torch.int64).contiguous()
         _lib.check(lib.tdiff_set_ligand(eng, _ptr(lpos), _ptr(lv), mode, st))
         S, K = int(num_steps), self.num_classes
+        bits = None
+        if allowed_types is not None:
+            am = torch.as_tensor(allowed_types).detach().to(dev)
+            if am.dtype != torch.bool or tuple(am.shape) != (Nl, K):
+                raise ValueError('allowed_types must be a [Nl, K] = %s bool tensor, got %s %s' % ((Nl, K), tuple(am.shape), am.dtype))
+            bits = (am.to(torch.int32) << torch.arange(K, dtype=torch.int32, device=dev)).sum(1, dtype=torch.int32).contiguous()
+        _lib.check(lib.tdiff_set_type_mask(eng, _ptr(bits), st))                # None clears: a call never inherits a mask
         pos_noise = v_uniform = None
         if noise_tape is not None:
             pos_noise = noise_tape[0].detach().to(dev, torch.float32).contiguous()
