@@ -28,7 +28,56 @@ __device__ __forceinline__ float log_add_exp_f(float a, float b) {
   return mx + logf(expf(a - mx) + expf(b - mx));
 }
 
-// Philox domain words of the fixed-atom stream ("fxps", "fxtv"), distinct from the sampler's "pst\0" / "vuni" (oracle/fixed_atoms.py)
+#define TD_LOG_EPS (-69.07755279f)   // logf(1e-30f): index_to_log_onehot's clamp (reference :124-130)
+
+// log_add_exp(log_onehot(v)[c] + lam, l1m): class c's term of q(. | onehot(v)) in log space, the unnormalised form of q_v_pred and
+// q_v_pred_one_timestep (reference :371-392)
+__device__ __forceinline__ float log_q_onehot(int c, int v, float lam, float l1m) {
+  return log_add_exp_f(((c == v) ? 0.0f : TD_LOG_EPS) + lam, l1m);
+}
+
+// lr = log_softmax of the type head's row lg[0 .. K); with kMask, the classes whose bit of `am` is clear enter as -inf (exp gives exactly
+// 0 there, so every sum is unchanged when all are allowed) and leave as -inf
+template <bool kMask>
+__device__ __forceinline__ void log_softmax(const float* lg, int K, uint32_t am, float* lr) {
+  float mx = -INFINITY;
+  for (int c = 0; c < K; ++c) {
+    lr[c] = (kMask && !((am >> c) & 1u)) ? -INFINITY : lg[c];
+    mx = fmaxf(mx, lr[c]);
+  }
+  float se = 0.0f;
+  for (int c = 0; c < K; ++c) se += expf(lr[c] - mx);
+  const float lse = logf(se);
+  for (int c = 0; c < K; ++c) lr[c] = (lr[c] - mx) - lse;
+}
+
+// One class of a Gumbel-max draw (log_sample_categorical, reference :160-166): class c with uniform u and log-probability lp replaces
+// the best so far only on a strictly larger score, so that a tie goes to the lowest class, as the reference's argmax does
+__device__ __forceinline__ void gumbel_max(float u, float lp, int c, float& best, int& vbest) {
+  const float sc = -logf(-logf(u + 1e-30f) + 1e-30f) + lp;
+  if (sc > best) { best = sc; vbest = c; }
+}
+
+// c x + d eps with every product and the sum rounded once, as the reference's perturbation (models/molopt_score_model.py:500-504)
+__device__ __forceinline__ float4 forward_transition(float c, float d, const float4& x, const float nz[3]) {
+  return make_float4(__fadd_rn(__fmul_rn(c, x.x), __fmul_rn(d, nz[0])), __fadd_rn(__fmul_rn(c, x.y), __fmul_rn(d, nz[1])),
+                     __fadd_rn(__fmul_rn(c, x.z), __fmul_rn(d, nz[2])), 1.0f);
+}
+
+// Row s of the trajectories: pos_traj the centred x plus the graph's offset, v_traj the class v
+__device__ __forceinline__ void write_traj(const TdStepArgs& A, int s, int a, const float4& x, int v) {
+  if (A.pos_traj) {
+    const float4 off = A.offset[A.lig_graph[a]];
+    float* o = A.pos_traj + ((size_t)s * A.n_lig + a) * 3;
+    o[0] = x.x + off.x; o[1] = x.y + off.y; o[2] = x.z + off.z;
+  }
+  if (A.v_traj) A.v_traj[(size_t)s * A.n_lig + a] = (long long)v;
+}
+
+// Philox domain words of the sampling chain's own stream ("pst\0", "vuni"; oracle/philox.py)
+#define TD_STEP_POS_DOMAIN 0x70737400u
+#define TD_STEP_TYPE_DOMAIN 0x76756e69u
+// Philox domain words of the fixed-atom stream ("fxps", "fxtv"), distinct from the two above (oracle/fixed_atoms.py)
 #define TD_FIX_POS_DOMAIN 0x66787073u
 #define TD_FIX_TYPE_DOMAIN 0x66787476u
 // Philox domain words of the start-ligand stream ("stps", "sttv"), distinct from the four above (oracle/start_ligand.py)
@@ -39,13 +88,21 @@ __device__ __forceinline__ float log_add_exp_f(float a, float b) {
 #define TD_LK_POS_DOMAIN 0x6c6b7073u
 #define TD_LK_TYPE_DOMAIN 0x6c6b7476u
 
-// Draw layout of forward_sample: tape row `d * Nl + a` and Philox counter (a, d, lane, domain), lane 0 for positions and 1 + c/4 for
-// class c -- the fixed-atom and start streams'
+// A random stream (Src) names its tapes, its Philox domain words and its draw layout: the tape row of draw d of row a, and its counter,
+// lane 0 for positions and 1 + c/4 for class c.  TdDrawByRow is the layout of the step, fixed-atom and start streams: tape row
+// d * Nl + a and counter (a, d, lane, domain).
 struct TdDrawByRow {
   static __device__ __forceinline__ size_t row(const TdStepArgs& A, int a, int d) { return (size_t)d * A.n_lig + a; }
   static __device__ __forceinline__ uint4 counter(const TdStepArgs&, int a, int d, unsigned lane, unsigned domain) {
     return make_uint4((unsigned)a, (unsigned)d, lane, domain);
   }
+};
+
+// The chain's own stream: draw d = s is step s (steps already taken), whichever its kind (DESIGN.md section 1)
+struct TdStepSource : TdDrawByRow {
+  static constexpr unsigned kPosDomain = TD_STEP_POS_DOMAIN, kTypeDomain = TD_STEP_TYPE_DOMAIN;
+  static __device__ __forceinline__ const float* pos_tape(const TdStepArgs& A) { return A.pos_noise; }
+  static __device__ __forceinline__ const float* v_tape(const TdStepArgs& A) { return A.v_uniform; }
 };
 
 // Sources of forward_sample: x0 / v0, the tapes and the Philox domain words of the fixed-atom stream and of the start stream
@@ -78,11 +135,44 @@ struct TdLikelihoodSource {
   }
 };
 
-// Row `a`: a sample of q(x_tm | x0) and q(v_tm | v0) with x0 / v0 from `Src`, from draw `d` of its stream (the sampler's key, Src's
-// counter layout and domain words) or row Src::row(a, d) of its tapes [., 3] / [., K]; x0 / v0 exactly when tm < 0.  Position
-// sqrt(ac) x0 + sqrt(1 - ac) eps with every product and the sum rounded once, as the reference's perturbation
-// (models/molopt_score_model.py:500-504); type: Gumbel-max over the unnormalised q_v_pred(log_onehot(v0), tm) (q_v_sample, :394-398).
-// With pos_only the type is left as it is.
+// Every random number of the sampler is drawn by draw_normal3 and draw_uniform4, from draw d of row a of the stream Src: a tape row, or
+// Philox4x32-10 on Src's counter under the sampler's key (seed mod 2^32, seed >> 32).
+template <class Src>
+__device__ __forceinline__ uint4 philox_draw(const TdStepArgs& A, int a, int d, unsigned lane, unsigned domain) {
+  return philox4x32_10(Src::counter(A, a, d, lane, domain), make_uint2((unsigned)A.seed, (unsigned)(A.seed >> 32)));
+}
+// nz = three standard normals: row Src::row(a, d) of the position tape [., 3], or Box-Muller on counter (a, d, 0, position domain) with
+// u0, u2 in (0, 1] and u1, u3 in [0, 1).
+template <class Src>
+__device__ __forceinline__ void draw_normal3(const TdStepArgs& A, int a, int d, float nz[3]) {
+  if (Src::pos_tape(A)) {
+    const float* pn = Src::pos_tape(A) + Src::row(A, a, d) * 3;
+    nz[0] = pn[0]; nz[1] = pn[1]; nz[2] = pn[2];
+  } else {
+    const uint4 r0 = philox_draw<Src>(A, a, d, 0u, Src::kPosDomain);
+    const float u0 = 1.0f - u01(r0.x), u1 = u01(r0.y), u2 = 1.0f - u01(r0.z), u3 = u01(r0.w);
+    const float ra = sqrtf(-2.0f * logf(u0)), rb = sqrtf(-2.0f * logf(u2));
+    nz[0] = ra * cospif(2.0f * u1); nz[1] = ra * sinpif(2.0f * u1); nz[2] = rb * cospif(2.0f * u3);
+  }
+}
+// u[j] = the uniform of class c0 + j (c0 a multiple of 4): the type tape [., K] for c0 + j < K, or the four words of counter
+// (a, d, 1 + c0/4, type domain)
+template <class Src>
+__device__ __forceinline__ void draw_uniform4(const TdStepArgs& A, int a, int d, int c0, float u[4]) {
+  const int K = A.n_classes;
+  if (Src::v_tape(A)) {
+    const float* vu = Src::v_tape(A) + Src::row(A, a, d) * K;
+    for (int j = 0; j < 4 && c0 + j < K; ++j) u[j] = vu[c0 + j];
+  } else {
+    const uint4 r = philox_draw<Src>(A, a, d, 1u + (unsigned)(c0 >> 2), Src::kTypeDomain);
+    u[0] = u01(r.x); u[1] = u01(r.y); u[2] = u01(r.z); u[3] = u01(r.w);
+  }
+}
+
+// Row `a`: a sample of q(x_tm | x0) and q(v_tm | v0) with x0 / v0 from `Src`, from draw `d` of its stream or tapes; x0 / v0 exactly
+// when tm < 0.  Position sqrt(ac) x0 + sqrt(1 - ac) eps (forward_transition); type: Gumbel-max over the unnormalised
+// q_v_pred(log_onehot(v0), tm) (q_v_sample, :394-398).  With pos_only the type is left as it is.  For a fixed atom (TdFixedSource,
+// DESIGN.md section 1) d = 0 is the draw before the first step and d = j + 1 the draw after step j.
 template <class Src>
 __device__ __forceinline__ void forward_sample(const TdStepArgs& A, int a, int d, int tm, float4& x, int& v) {
   const float4 x0 = Src::x0(A)[a];
@@ -91,52 +181,21 @@ __device__ __forceinline__ void forward_sample(const TdStepArgs& A, int a, int d
     if (!A.pos_only) v = Src::v0(A)[a];
     return;
   }
-  const uint2 key = make_uint2((unsigned)A.seed, (unsigned)(A.seed >> 32));
   float nz[3];
-  if (Src::pos_tape(A)) {
-    const float* pn = Src::pos_tape(A) + Src::row(A, a, d) * 3;
-    nz[0] = pn[0]; nz[1] = pn[1]; nz[2] = pn[2];
-  } else {
-    const uint4 r0 = philox4x32_10(Src::counter(A, a, d, 0u, Src::kPosDomain), key);
-    const float u0 = 1.0f - u01(r0.x), u1 = u01(r0.y), u2 = 1.0f - u01(r0.z), u3 = u01(r0.w);
-    const float ra = sqrtf(-2.0f * logf(u0)), rb = sqrtf(-2.0f * logf(u2));
-    nz[0] = ra * cospif(2.0f * u1); nz[1] = ra * sinpif(2.0f * u1); nz[2] = rb * cospif(2.0f * u3);
-  }
+  draw_normal3<Src>(A, a, d, nz);
   const float acv = A.ac[tm];
-  const float sa = sqrtf(acv), sb = sqrtf(1.0f - acv);
-  x.x = __fadd_rn(__fmul_rn(sa, x0.x), __fmul_rn(sb, nz[0]));
-  x.y = __fadd_rn(__fmul_rn(sa, x0.y), __fmul_rn(sb, nz[1]));
-  x.z = __fadd_rn(__fmul_rn(sa, x0.z), __fmul_rn(sb, nz[2]));
-  x.w = 1.0f;
+  x = forward_transition(sqrtf(acv), sqrtf(1.0f - acv), x0, nz);
   if (A.pos_only) return;
   const int K = A.n_classes, v0 = Src::v0(A)[a];
   const float lca = A.lca_v[tm], l1mca = A.l1mca_v[tm] - A.log_k;
-  const float log_eps = -69.07755279f;                                     // logf(1e-30f): index_to_log_onehot's clamp
   float best = -INFINITY;
   int vbest = 0;
   for (int c0 = 0; c0 < K; c0 += 4) {
     float u[4];
-    if (Src::v_tape(A)) {
-      const float* vu = Src::v_tape(A) + Src::row(A, a, d) * K;
-      for (int j = 0; j < 4 && c0 + j < K; ++j) u[j] = vu[c0 + j];
-    } else {
-      const uint4 r = philox4x32_10(Src::counter(A, a, d, 1u + (unsigned)(c0 >> 2), Src::kTypeDomain), key);
-      u[0] = u01(r.x); u[1] = u01(r.y); u[2] = u01(r.z); u[3] = u01(r.w);
-    }
-    for (int j = 0; j < 4 && c0 + j < K; ++j) {
-      const int c = c0 + j;
-      const float lp = log_add_exp_f(((c == v0) ? 0.0f : log_eps) + lca, l1mca);
-      const float sc = -logf(-logf(u[j] + 1e-30f) + 1e-30f) + lp;
-      if (sc > best) { best = sc; vbest = c; }
-    }
+    draw_uniform4<Src>(A, a, d, c0, u);
+    for (int j = 0; j < 4 && c0 + j < K; ++j) gumbel_max(u[j], log_q_onehot(c0 + j, v0, lca, l1mca), c0 + j, best, vbest);
   }
   v = vbest;
-}
-
-// Fixed atom `a` (DESIGN.md section 1, fixed atoms): a sample of q(x_tm | x0_f) and q(v_tm | v0_f) from draw `d` of the fixed-atom
-// stream or tape (d = 0 before the first step, d = j + 1 after step j), or x0_f / v0_f exactly when tm < 0.
-__device__ __forceinline__ void fixed_sample(const TdStepArgs& A, int a, int d, int tm, float4& x, int& v) {
-  forward_sample<TdFixedSource>(A, a, d, tm, x, v);
 }
 
 // The step's x0 prediction of ligand row `a` at network time t, centred frame: the node array's row in C0 mode; in 'noise' mode
@@ -153,15 +212,14 @@ __device__ __forceinline__ float4 td_pred_x0(const TdStepArgs& A, int a, int t, 
   return x0;
 }
 
-// kFixed = false (no fixed set) compiles to the step as it was before fixed atoms existed.  kSeq = true runs step s of a respaced
-// chain (DESIGN.md section 1): the network saw t = seq_t[s], and the state moves to p = seq_p[s] with the per-step coefficients
-// seq_*[s]; kSeq = false is the default chain t = t_start - s, p = t - 1 on the checkpoint's tables.  A guided step (clash guidance)
-// runs these same instances with xm_final = the guided predictions and mean_noise = 0: the guidance kernel has already converted them.
-// kMask = true (element constraints, DESIGN.md section 1): bit c of allowed[a] set = class c allowed for row a.  The type head's
-// log_softmax runs over the allowed classes only (the others enter as -inf, so exp gives exactly 0 and every sum is unchanged when all
-// are allowed), and on the decoder step (p < 0) the posterior's forbidden classes are -inf before its normalisation, so that it is
-// renormalised over the allowed set and the Gumbel-max draw can only pick an allowed class.  kMask = false never reads `allowed`.
-template <bool kFixed, bool kSeq, bool kMask>
+// kSeq = true runs step s of a respaced chain (DESIGN.md section 1): the network saw t = seq_t[s], and the state moves to p = seq_p[s]
+// with the per-step coefficients seq_*[s]; kSeq = false is the default chain t = t_start - s, p = t - 1 on the checkpoint's tables.  A
+// guided step (clash guidance) runs these same instances with xm_final = the guided predictions and mean_noise = 0: the guidance kernel
+// has already converted them.  kMask = true (element constraints, DESIGN.md section 1): bit c of allowed[a] set = class c allowed for
+// row a.  The type head's log_softmax runs over the allowed classes only, and on the decoder step (p < 0) the posterior's forbidden
+// classes are -inf before its normalisation, so that it is renormalised over the allowed set and the Gumbel-max draw can only pick an
+// allowed class.  kMask = false never reads `allowed`.  Fixed rows (fix_mask) are overwritten after the update.
+template <bool kSeq, bool kMask>
 __global__ void step_epilogue_kernel(TdStepArgs A, const uint32_t* __restrict__ allowed) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a >= A.n_lig) return;
@@ -169,40 +227,11 @@ __global__ void step_epilogue_kernel(TdStepArgs A, const uint32_t* __restrict__ 
   const int t = kSeq ? A.seq_t[s] : A.t_start - s;   // current timestep (reference :649-651)
   const int p = kSeq ? A.seq_p[s] : t - 1;           // the time this step moves to
   const int K = A.n_classes;
-  const bool fixed = kFixed && A.fix_mask[a];
-
-  // noise for this atom
-  float nz[3];
-  float un[TD_CMAX];
-  if (A.pos_noise) {
-    const float* pn = A.pos_noise + ((size_t)s * A.n_lig + a) * 3;
-    nz[0] = pn[0]; nz[1] = pn[1]; nz[2] = pn[2];
-  } else {
-    const uint2 key = make_uint2((unsigned)A.seed, (unsigned)(A.seed >> 32));
-    const uint4 r0 = philox4x32_10(make_uint4((unsigned)a, (unsigned)s, 0u, 0x70737400u), key);
-    // Box-Muller on (0,1] uniforms
-    const float u0 = 1.0f - u01(r0.x), u1 = u01(r0.y), u2 = 1.0f - u01(r0.z), u3 = u01(r0.w);
-    const float ra = sqrtf(-2.0f * logf(u0)), rb = sqrtf(-2.0f * logf(u2));
-    nz[0] = ra * cospif(2.0f * u1); nz[1] = ra * sinpif(2.0f * u1); nz[2] = rb * cospif(2.0f * u3);
-  }
-  if (!A.pos_only) {
-    if (A.v_uniform) {
-      const float* vu = A.v_uniform + ((size_t)s * A.n_lig + a) * K;
-      for (int c = 0; c < K; ++c) un[c] = vu[c];
-    } else {
-      const uint2 key = make_uint2((unsigned)A.seed, (unsigned)(A.seed >> 32));
-      for (int c0 = 0; c0 < K; c0 += 4) {
-        const uint4 r = philox4x32_10(make_uint4((unsigned)a, (unsigned)s, 1u + (unsigned)(c0 >> 2), 0x76756e69u), key);
-        un[c0] = u01(r.x);
-        if (c0 + 1 < K) un[c0 + 1] = u01(r.y);
-        if (c0 + 2 < K) un[c0 + 2] = u01(r.z);
-        if (c0 + 3 < K) un[c0 + 3] = u01(r.w);
-      }
-    }
-  }
+  const bool fixed = A.fix_mask && A.fix_mask[a];
 
   // ---- positions: posterior mean + noise (reference :673-679)
-  const int g = A.lig_graph[a];
+  float nz[3];
+  draw_normal3<TdStepSource>(A, a, s, nz);
   const float4 xt = A.lig_pos[a];
   const float4 x0 = td_pred_x0(A, a, t, xt);
   const float c0 = kSeq ? A.seq_c0[s] : A.c0[t], ct = kSeq ? A.seq_ct[s] : A.ct[t];
@@ -214,39 +243,23 @@ __global__ void step_epilogue_kernel(TdStepArgs A, const uint32_t* __restrict__ 
   xn.w = 1.0f;
   // a fixed row is overwritten after the update: q(x_p | x0_f) from draw s + 1, or x0_f itself after t = 0
   int vfix = 0;
-  if (fixed) fixed_sample(A, a, s + 1, p, xn, vfix);
+  if (fixed) forward_sample<TdFixedSource>(A, a, s + 1, p, xn, vfix);
   A.lig_pos[a] = xn;
-  const float4 off = A.offset[g];
-  if (A.pos_traj) {
-    float* o = A.pos_traj + ((size_t)s * A.n_lig + a) * 3;
-    o[0] = xn.x + off.x; o[1] = xn.y + off.y; o[2] = xn.z + off.z;
-  }
 
   int vnew = A.lig_v[a];
   if (!A.pos_only) {
     // ---- atom types: categorical posterior in log space (reference :682-685)
-    const float* lg = A.logits + (size_t)a * K;
     float lr[TD_CMAX];
-    float mx = -INFINITY;
     const uint32_t am = kMask ? allowed[a] : 0u;
-    for (int c = 0; c < K; ++c) {
-      lr[c] = (kMask && !((am >> c) & 1u)) ? -INFINITY : lg[c];
-      mx = fmaxf(mx, lr[c]);
-    }
-    float se = 0.0f;
-    for (int c = 0; c < K; ++c) se += expf(lr[c] - mx);
-    const float lse = logf(se);
-    for (int c = 0; c < K; ++c) lr[c] = (lr[c] - mx) - lse;                 // log_softmax
+    log_softmax<kMask>(A.logits + (size_t)a * K, K, am, lr);
     const int tm1 = kSeq ? (p > 0 ? p : 0) : (t > 0 ? t - 1 : 0);
     const float lca = A.lca_v[tm1], l1mca = A.l1mca_v[tm1] - A.log_k;
     const float la = kSeq ? A.seq_la[s] : A.la_v[t], l1ma = (kSeq ? A.seq_l1ma[s] : A.l1ma_v[t]) - A.log_k;
     const int vcur = vnew;
-    const float log_eps = -69.07755279f;                                   // logf(1e-30f)
     float un_lp[TD_CMAX];
     float m2 = -INFINITY;
     for (int c = 0; c < K; ++c) {
-      const float lvt = (c == vcur) ? 0.0f : log_eps;
-      un_lp[c] = log_add_exp_f(lr[c] + lca, l1mca) + log_add_exp_f(lvt + la, l1ma);
+      un_lp[c] = log_add_exp_f(lr[c] + lca, l1mca) + log_q_onehot(c, vcur, la, l1ma);
       if (kMask && p < 0 && !((am >> c) & 1u)) un_lp[c] = -INFINITY;       // decoder step: renormalised over the allowed set
       m2 = fmaxf(m2, un_lp[c]);
     }
@@ -257,31 +270,29 @@ __global__ void step_epilogue_kernel(TdStepArgs A, const uint32_t* __restrict__ 
     vnew = 0;
     float* o0 = A.v0_traj ? A.v0_traj + ((size_t)s * A.n_lig + a) * K : nullptr;
     float* ot = A.vt_traj ? A.vt_traj + ((size_t)s * A.n_lig + a) * K : nullptr;
-    for (int c = 0; c < K; ++c) {
-      const float lp = un_lp[c] - lse2;
-      const float gum = -logf(-logf(un[c] + 1e-30f) + 1e-30f);
-      const float sc = gum + lp;
-      if (sc > best) { best = sc; vnew = c; }
-      if (o0) o0[c] = lr[c];
-      if (ot) ot[c] = lp;
+    for (int c0 = 0; c0 < K; c0 += 4) {
+      float u[4];
+      draw_uniform4<TdStepSource>(A, a, s, c0, u);
+      for (int j = 0; j < 4 && c0 + j < K; ++j) {
+        const int c = c0 + j;
+        const float lp = un_lp[c] - lse2;
+        gumbel_max(u[j], lp, c, best, vnew);
+        if (o0) o0[c] = lr[c];
+        if (ot) ot[c] = lp;
+      }
     }
     if (fixed) vnew = vfix;                    // v0_traj / vt_traj above keep the model's own opinion of the row
     A.lig_v[a] = vnew;
   }
-  if (A.v_traj) A.v_traj[(size_t)s * A.n_lig + a] = (long long)vnew;
+  write_traj(A, s, a, xn, vnew);
 }
 
 __global__ void advance_step_kernel(int* step) { *step += 1; }
 
 template <bool kMask>
 static void launch_step_epilogue(const TdStepArgs& A, const uint32_t* allowed, int grid, cudaStream_t st) {
-  if (A.seq_t) {
-    if (A.fix_mask) step_epilogue_kernel<true, true, kMask><<<grid, 128, 0, st>>>(A, allowed);
-    else step_epilogue_kernel<false, true, kMask><<<grid, 128, 0, st>>>(A, allowed);
-  } else {
-    if (A.fix_mask) step_epilogue_kernel<true, false, kMask><<<grid, 128, 0, st>>>(A, allowed);
-    else step_epilogue_kernel<false, false, kMask><<<grid, 128, 0, st>>>(A, allowed);
-  }
+  if (A.seq_t) step_epilogue_kernel<true, kMask><<<grid, 128, 0, st>>>(A, allowed);
+  else step_epilogue_kernel<false, kMask><<<grid, 128, 0, st>>>(A, allowed);
 }
 void td_launch_step_epilogue(const TdStepArgs& A, const uint32_t* allowed, cudaStream_t st) {
   if (A.n_lig > 0) {
@@ -362,50 +373,34 @@ void td_launch_clash_guidance(const TdStepArgs& A, const TdGuideArgs& G, int n_g
 // Re-noising step s of a time path (tdiff_sample_path, DESIGN.md section 1): the state moves up from t = seq_t[s] to p = seq_p[s] > t
 // with the forward process, no network.  The step tables hold c = sqrt(abar_p / abar_t) in seq_c0, d = sqrt(1 - abar_p / abar_t) in
 // seq_ct, lambda = log of the type schedule's transition probability t -> p in seq_la and log(1 - e^lambda + 1e-40) in seq_l1ma.  A row
-// that is not fixed: x_p = c x_t + d eps with each product and the sum rounded once (forward_sample's roundings), and a Gumbel-max
-// draw over the unnormalised log q(v_p | v_t) = log_add_exp(log_onehot(v_t) + lambda, l1ma - log K) (q_v_sample's form); with pos_only
-// the type stays.  Fixed rows: q(x_p | x0_f), q(v_p | v0_f) from draw s + 1, as after a denoising step.  The random stream is the
-// denoising step's: row s of the tapes, or counters (a, s, 0, "pst\0") and (a, s, 1 + c/4, "vuni").  Trajectories: pos_traj / v_traj
-// the new state, vt_traj the normalised log q(v_p | v_t), v0_traj a copy of entry s - 1 (the latest network prediction).
-template <bool kFixed>
+// that is not fixed: x_p = c x_t + d eps (forward_transition), and a Gumbel-max draw over the unnormalised log q(v_p | v_t) =
+// log_add_exp(log_onehot(v_t) + lambda, l1ma - log K) (q_v_sample's form); with pos_only the type stays.  Fixed rows: q(x_p | x0_f),
+// q(v_p | v0_f) from draw s + 1, as after a denoising step.  The random stream is the denoising step's, draw s of TdStepSource.
+// Trajectories: pos_traj / v_traj the new state, vt_traj the normalised log q(v_p | v_t), v0_traj a copy of entry s - 1 (the latest
+// network prediction).
 __global__ void renoise_kernel(TdStepArgs A) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x;
   if (a >= A.n_lig) return;
   const int s = *A.step;
   const int p = A.seq_p[s];
   const int K = A.n_classes;
-  const bool fixed = kFixed && A.fix_mask[a];
-  const uint2 key = make_uint2((unsigned)A.seed, (unsigned)(A.seed >> 32));
+  const bool fixed = A.fix_mask && A.fix_mask[a];
   float4 xn;
   int vnew = A.lig_v[a];
   if (!fixed) {
     float nz[3];
-    if (A.pos_noise) {
-      const float* pn = A.pos_noise + ((size_t)s * A.n_lig + a) * 3;
-      nz[0] = pn[0]; nz[1] = pn[1]; nz[2] = pn[2];
-    } else {
-      const uint4 r0 = philox4x32_10(make_uint4((unsigned)a, (unsigned)s, 0u, 0x70737400u), key);
-      const float u0 = 1.0f - u01(r0.x), u1 = u01(r0.y), u2 = 1.0f - u01(r0.z), u3 = u01(r0.w);
-      const float ra = sqrtf(-2.0f * logf(u0)), rb = sqrtf(-2.0f * logf(u2));
-      nz[0] = ra * cospif(2.0f * u1); nz[1] = ra * sinpif(2.0f * u1); nz[2] = rb * cospif(2.0f * u3);
-    }
-    const float4 xt = A.lig_pos[a];
-    const float c = A.seq_c0[s], d = A.seq_ct[s];
-    xn.x = __fadd_rn(__fmul_rn(c, xt.x), __fmul_rn(d, nz[0]));
-    xn.y = __fadd_rn(__fmul_rn(c, xt.y), __fmul_rn(d, nz[1]));
-    xn.z = __fadd_rn(__fmul_rn(c, xt.z), __fmul_rn(d, nz[2]));
-    xn.w = 1.0f;
+    draw_normal3<TdStepSource>(A, a, s, nz);
+    xn = forward_transition(A.seq_c0[s], A.seq_ct[s], A.lig_pos[a], nz);
   } else {
-    fixed_sample(A, a, s + 1, p, xn, vnew);
+    forward_sample<TdFixedSource>(A, a, s + 1, p, xn, vnew);
   }
   if (!A.pos_only) {
     const float la = A.seq_la[s], l1ma = A.seq_l1ma[s] - A.log_k;
-    const float log_eps = -69.07755279f;                                   // logf(1e-30f): index_to_log_onehot's clamp
     const int vcur = A.lig_v[a];
     float lq[TD_CMAX];
     float mx = -INFINITY;
     for (int c = 0; c < K; ++c) {
-      lq[c] = log_add_exp_f(((c == vcur) ? 0.0f : log_eps) + la, l1ma);
+      lq[c] = log_q_onehot(c, vcur, la, l1ma);
       mx = fmaxf(mx, lq[c]);
     }
     float se = 0.0f;
@@ -418,17 +413,10 @@ __global__ void renoise_kernel(TdStepArgs A) {
     int vbest = 0;
     for (int c0 = 0; c0 < K; c0 += 4) {
       float u[4];
-      if (A.v_uniform) {
-        const float* vu = A.v_uniform + ((size_t)s * A.n_lig + a) * K;
-        for (int j = 0; j < 4 && c0 + j < K; ++j) u[j] = vu[c0 + j];
-      } else {
-        const uint4 r = philox4x32_10(make_uint4((unsigned)a, (unsigned)s, 1u + (unsigned)(c0 >> 2), 0x76756e69u), key);
-        u[0] = u01(r.x); u[1] = u01(r.y); u[2] = u01(r.z); u[3] = u01(r.w);
-      }
+      draw_uniform4<TdStepSource>(A, a, s, c0, u);
       for (int j = 0; j < 4 && c0 + j < K; ++j) {
         const int c = c0 + j;
-        const float sc = -logf(-logf(u[j] + 1e-30f) + 1e-30f) + lq[c];
-        if (sc > best) { best = sc; vbest = c; }
+        gumbel_max(u[j], lq[c], c, best, vbest);
         if (ot) ot[c] = lq[c] - lse;
         if (o0) o0[c] = p0[c];
       }
@@ -437,20 +425,11 @@ __global__ void renoise_kernel(TdStepArgs A) {
     A.lig_v[a] = vnew;
   }
   A.lig_pos[a] = xn;
-  if (A.pos_traj) {
-    const float4 off = A.offset[A.lig_graph[a]];
-    float* o = A.pos_traj + ((size_t)s * A.n_lig + a) * 3;
-    o[0] = xn.x + off.x; o[1] = xn.y + off.y; o[2] = xn.z + off.z;
-  }
-  if (A.v_traj) A.v_traj[(size_t)s * A.n_lig + a] = (long long)vnew;
+  write_traj(A, s, a, xn, vnew);
 }
 
 void td_launch_renoise(const TdStepArgs& A, cudaStream_t st) {
-  if (A.n_lig > 0) {
-    const int grid = (A.n_lig + 127) / 128;
-    if (A.fix_mask) renoise_kernel<true><<<grid, 128, 0, st>>>(A);
-    else renoise_kernel<false><<<grid, 128, 0, st>>>(A);
-  }
+  if (A.n_lig > 0) renoise_kernel<<<(A.n_lig + 127) / 128, 128, 0, st>>>(A);
   advance_step_kernel<<<1, 1, 0, st>>>(A.step);
 }
 
@@ -460,7 +439,7 @@ __global__ void fixed_init_kernel(TdStepArgs A) {
   if (a >= A.n_lig || !A.fix_mask[a]) return;
   float4 x;
   int v = A.lig_v[a];
-  fixed_sample(A, a, 0, A.t_start, x, v);
+  forward_sample<TdFixedSource>(A, a, 0, A.t_start, x, v);
   A.lig_pos[a] = x;
   A.lig_v[a] = v;
 }
@@ -476,7 +455,7 @@ __global__ void start_init_kernel(TdStepArgs A) {
   if (a >= A.n_lig) return;
   float4 x;
   int v = A.lig_v[a];
-  if (A.fix_mask && A.fix_mask[a]) fixed_sample(A, a, 0, A.t_start, x, v);
+  if (A.fix_mask && A.fix_mask[a]) forward_sample<TdFixedSource>(A, a, 0, A.t_start, x, v);
   else forward_sample<TdStartSource>(A, a, 0, A.t_start, x, v);
   A.lig_pos[a] = x;
   A.lig_v[a] = v;
@@ -519,7 +498,6 @@ __global__ void __launch_bounds__(128) likelihood_epilogue_kernel(TdLikelihoodAr
   const int g = blockIdx.x, tid = threadIdx.x;
   const int b = L.node_ptr[g] - L.prot_ptr[g], e = L.node_ptr[g + 1] - L.prot_ptr[g + 1];
   const int t = A.lk_t[g], T = L.n_timesteps, K = A.n_classes;
-  const float log_eps = -69.07755279f;                                     // logf(1e-30f): index_to_log_onehot's clamp
   const float log_sqrt_2pi = 0.918938533f;                                 // np.log(np.sqrt(2 * np.pi)) in fp32
   const float log_2 = 0.693147181f;                                        // np.log(2.) in fp32
   float sum[4] = {0.f, 0.f, 0.f, 0.f};
@@ -549,22 +527,16 @@ __global__ void __launch_bounds__(128) likelihood_epilogue_kernel(TdLikelihoodAr
         tp = -lp;
       }
       // ---- types: q_v_posterior of log_softmax(logits) and of log_onehot(v0) given v_t (:401-409), at t - 1 clamped to 0
-      const float* lg = L.logits + (size_t)a * K;
       float lr[TD_CMAX], um[TD_CMAX], ut[TD_CMAX];
-      float mx = -INFINITY;
-      for (int c = 0; c < K; ++c) { lr[c] = lg[c]; mx = fmaxf(mx, lr[c]); }
-      float se = 0.0f;
-      for (int c = 0; c < K; ++c) se += expf(lr[c] - mx);
-      const float lse = logf(se);
-      for (int c = 0; c < K; ++c) lr[c] = (lr[c] - mx) - lse;
+      log_softmax<false>(L.logits + (size_t)a * K, K, 0u, lr);
       const int tm1 = t > 0 ? t - 1 : 0;
       const float lca = A.lca_v[tm1], l1mca = A.l1mca_v[tm1] - A.log_k;
       const float la = L.la_v[t], l1ma = L.l1ma_v[t] - A.log_k;
       float mm = -INFINITY, mt = -INFINITY;
       for (int c = 0; c < K; ++c) {
-        const float q1 = log_add_exp_f(((c == vt) ? 0.0f : log_eps) + la, l1ma);
+        const float q1 = log_q_onehot(c, vt, la, l1ma);
         um[c] = log_add_exp_f(lr[c] + lca, l1mca) + q1;
-        ut[c] = log_add_exp_f(((c == v0) ? 0.0f : log_eps) + lca, l1mca) + q1;
+        ut[c] = log_q_onehot(c, v0, lca, l1mca) + q1;
         mm = fmaxf(mm, um[c]); mt = fmaxf(mt, ut[c]);
       }
       float sm = 0.f, st = 0.f;
@@ -577,7 +549,7 @@ __global__ void __launch_bounds__(128) likelihood_epilogue_kernel(TdLikelihoodAr
           tv += __fmul_rn(expf(lt), lt - (um[c] - lsm));
         }
       } else {                     // -log_categorical(log_onehot(v0), log_model): the clamped entries weigh exp(log 1e-30)
-        const float w_eps = expf(log_eps);
+        const float w_eps = expf(TD_LOG_EPS);
         for (int c = 0; c < K; ++c) tv += __fmul_rn((c == v0) ? 1.0f : w_eps, um[c] - lsm);
         tv = -tv;
       }
@@ -592,7 +564,7 @@ __global__ void __launch_bounds__(128) likelihood_epilogue_kernel(TdLikelihoodAr
       const float lcaT = A.lca_v[T - 1], l1mcaT = A.l1mca_v[T - 1] - A.log_k, log_half = -logf((float)K);
       float pv = 0.f;
       for (int c = 0; c < K; ++c) {
-        const float lq = log_add_exp_f(((c == v0) ? 0.0f : log_eps) + lcaT, l1mcaT);
+        const float lq = log_q_onehot(c, v0, lcaT, l1mcaT);
         pv += __fmul_rn(expf(lq), lq - log_half);
       }
       terms[0][tid] = tp; terms[1][tid] = tv; terms[2][tid] = pp; terms[3][tid] = pv;

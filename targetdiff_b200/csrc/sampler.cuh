@@ -25,7 +25,7 @@ struct TdStepArgs {
   long long* v_traj;               // [S,Nl] or NULL
   float* v0_traj;                  // [S,Nl,K] or NULL
   float* vt_traj;                  // [S,Nl,K] or NULL
-  // fixed atoms (tdiff_set_fixed); fix_mask == NULL: none, and the kernel takes the default path only
+  // fixed atoms (tdiff_set_fixed); fix_mask == NULL: none
   const unsigned char* fix_mask;   // [Nl] 1 = the row is held to the forward process of (fix_pos, fix_v)
   const float4* fix_pos;           // [Nl] target positions x0_f, centred frame
   const int* fix_v;                // [Nl] target classes v0_f
