@@ -234,6 +234,25 @@ TDIFF_API int tdiff_sample_path(tdiff_engine* e, const int32_t* h_time_path, int
  * belongs to the handle: it refers to no batch rows, so it survives tdiff_bind_batch.  Off on a new handle. */
 TDIFF_API int tdiff_set_clash_guidance(tdiff_engine* e, float radius, float strength);
 
+/* Connectivity guidance (an extension beyond the reference, DESIGN.md section 1): at every denoising step of every following chain
+ * (tdiff_sample, tdiff_sample_seq, the denoising steps of tdiff_sample_path; after clash guidance when both are on), the step's x0
+ * predictions y of each graph's ligand atoms (centred frame) are moved so that the molecule's separate pieces come closer.  Ligand atoms
+ * a, c of a graph are bonded when |q_a - q_c| < radius, where q is y, or the target position x0_f for a fixed row (tdiff_set_fixed).
+ * With one connected component every atom keeps y bit for bit.  Otherwise each component C finds its closest outside pair (i in C,
+ * j not in C; smallest d = |q_i - q_j|, then the lowest within-graph (i, j)); a component with a fixed row stays, and every other one
+ * moves rigidly: each of its atoms gets y + f (q_j - q_i), f = (strength * w * (d - bond_length)) / d, w = 1 when j's component has a
+ * fixed row and 1/2 otherwise, all shifts from the unshifted predictions.  d^2 = (dx dx + dy dy) + dz dz, d = sqrt(d^2), every comparison,
+ * f and each coordinate of the shift are explicitly rounded fp32 operations, and every decision reads the graph's own atoms, so a graph
+ * gets the same bits in any batch.  The step then runs unchanged on the guided prediction; fixed rows keep their prediction and are
+ * overwritten as before.  No random numbers are drawn.  One more launch per denoising step; re-noising steps, tdiff_forward,
+ * tdiff_forward_blocks and tdiff_likelihood_terms ignore the setting.  A chain with more than TDIFF_CONNECT_MAX_ATOMS ligand atoms in a
+ * graph while guidance is on -> TDIFF_EINVAL before anything runs.  strength == 0 turns guidance off (radius and bond_length are then
+ * ignored); strength > 0 needs finite radius > 0 and 0 < bond_length < radius (Angstrom).  A negative or non-finite strength, or a bad
+ * radius or bond length with strength > 0 -> TDIFF_EINVAL and the previous setting stays.  The setting belongs to the handle: it
+ * survives tdiff_bind_batch.  Off on a new handle. */
+#define TDIFF_CONNECT_MAX_ATOMS 1024
+TDIFF_API int tdiff_set_connect_guidance(tdiff_engine* e, float radius, float bond_length, float strength);
+
 /* Element constraints (an extension beyond the reference, DESIGN.md section 1): d_allowed [Nl] uint32 (device), bit c of row a set =
  * class c allowed for ligand atom a.  At every denoising step of every following chain (tdiff_sample, tdiff_sample_seq, the denoising
  * steps of tdiff_sample_path, with or without clash guidance) the type head's log_softmax runs over the allowed classes only (the

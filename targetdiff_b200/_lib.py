@@ -56,6 +56,7 @@ SIGNATURES = {
     'tdiff_set_start': (_i, [_vp, _i, _vp, _vp]),
     'tdiff_sample_path': (_i, [_vp, _pi32, _i, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _i, _vp]),
     'tdiff_set_clash_guidance': (_i, [_vp, ctypes.c_float, ctypes.c_float]),
+    'tdiff_set_connect_guidance': (_i, [_vp, ctypes.c_float, ctypes.c_float, ctypes.c_float]),
     'tdiff_set_type_mask': (_i, [_vp, _vp, _vp]),
     'tdiff_likelihood_terms': (_i, [_vp, _pi32, ctypes.POINTER(ctypes.c_uint32), _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'tdiff_sample_host': (_i, [_vp, _i, _pi32, _pi32, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),

@@ -85,3 +85,32 @@ def type_violations(v, allowed):
     else:
         ok = torch.isin(v, a.long().reshape(-1))
     return int((~ok).sum())
+
+
+def ligand_components(pos, batch_ligand, radius):
+    """Per molecule g: the number of connected components of its atoms when atoms closer than `radius` are bonded, as an int64 [B]
+    tensor on the CPU (0 for a molecule without atoms), B = the number of molecules.  Computed in float64 on the CPU, for the
+    connectivity-guidance tests and timing tool; a distance criterion, not a chemical bond perception."""
+    p = torch.as_tensor(pos).detach().cpu().double()
+    bl = torch.as_tensor(batch_ligand).detach().cpu().long()
+    B = int(bl.max()) + 1 if bl.numel() else 0
+    out = torch.zeros(B, dtype=torch.int64)
+    for g in range(B):
+        x = p[bl == g]
+        n = len(x)
+        if n == 0:
+            continue
+        adj = (torch.cdist(x, x, compute_mode='donot_use_mm_for_euclid_dist') < float(radius)).numpy()
+        seen = np.zeros(n, dtype=bool)
+        for r in range(n):
+            if seen[r]:
+                continue
+            out[g] += 1
+            seen[r] = True
+            stack = [r]
+            while stack:
+                i = stack.pop()
+                nxt = np.nonzero(adj[i] & ~seen)[0]
+                seen[nxt] = True
+                stack.extend(nxt.tolist())
+    return out

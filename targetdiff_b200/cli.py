@@ -33,7 +33,9 @@ chain, with a --fragment or kept atoms only, and sample.pt also holds 'time_path
 commands run clash guidance (ScorePosNet3D.sample_diffusion), and the result also holds 'clash_guidance': {'radius', 'strength'}.  With
 `sample.allowed_elements: [C, N, O, ...]` or `sample.allowed_classes: [...]` (config.sample_allowed_classes, in the checkpoint's
 ligand_atom_mode) both commands constrain every free atom of the finished molecules to those classes, and the result also holds
-'allowed_classes'.  Molecule
+'allowed_classes'.  With `sample.connect_strength: lambda` > 0, `sample.connect_radius: rho` and `sample.connect_length: b`
+(config.sample_connect_guidance; strength 0, the default, is off) both commands run connectivity guidance, and the result also holds
+'connect_guidance': {'radius', 'length', 'strength'}.  Molecule
 reconstruction / SDF writing needs RDKit + OpenBabel and stays out of scope."""
 import argparse
 import os
@@ -42,8 +44,8 @@ import sys
 
 import torch
 
-from .config import (check_resampling, load_config, sample_allowed_classes, sample_clash_guidance, sampling_start, sampling_time_path,
-                     sampling_time_seq)
+from .config import (check_resampling, load_config, sample_allowed_classes, sample_clash_guidance, sample_connect_guidance, sampling_start,
+                     sampling_time_path, sampling_time_seq)
 from .likelihood import likelihood_time_steps, ligand_nll
 from .pocket import LIGAND_CLASS_ELEMENTS, pdb_to_pocket_data
 from .sampling import sample_diffusion_ligand, seed_all
@@ -78,6 +80,13 @@ def add_clash_guidance(result, radius, strength):
     """Record a clash-guidance setting in a result dict; nothing when guidance is off, so the file is as without it."""
     if strength > 0:
         result['clash_guidance'] = {'radius': radius, 'strength': strength}
+    return result
+
+
+def add_connect_guidance(result, radius, length, strength):
+    """Record a connectivity-guidance setting in a result dict; nothing when guidance is off, so the file is as without it."""
+    if strength > 0:
+        result['connect_guidance'] = {'radius': radius, 'length': length, 'strength': strength}
     return result
 
 
@@ -165,6 +174,7 @@ def sample_pockets(argv):
     sampling_start(config.sample, None, False)      # start ligands are sample_for_pocket's only: refuses sample.start_time
     check_resampling(config.sample, False)          # so is resampling, which needs held atoms: refuses sample.resamplings
     clash_radius, clash_strength = sample_clash_guidance(config.sample)
+    connect_radius, connect_length, connect_strength = sample_connect_guidance(config.sample)
     rank, world, local_rank = tdist.init_from_env()
     device = a.device or 'cuda:%d' % local_rank
     paths = list_pockets(a.pocket_dir, a.pocket_list)
@@ -184,8 +194,11 @@ def sample_pockets(argv):
         outputs = sample_diffusion_ligand(model, data, n, batch_size=a.batch_size, device=device, num_steps=num_steps,
                                           pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
                                           sample_num_atoms=config.sample.sample_num_atoms, time_seq=time_seq,
-                                          clash_radius=clash_radius, clash_strength=clash_strength, allowed_types=allowed)
+                                          clash_radius=clash_radius, clash_strength=clash_strength, allowed_types=allowed,
+                                          connect_radius=connect_radius, connect_length=connect_length, connect_strength=connect_strength)
         result = add_allowed_classes(add_clash_guidance(build_result(data, outputs), clash_radius, clash_strength), allowed)
+        result = add_connect_guidance(result, connect_radius, connect_length, connect_strength)
+        result = add_connect_guidance(result, connect_radius, connect_length, connect_strength)
         if time_seq is not None:
             result['time_seq'] = time_seq
         torch.save(result, os.path.join(a.result_path, 'result_%d.pt' % i))
@@ -254,6 +267,7 @@ def sample_for_pocket(argv):
     held = fragment is not None or (start is not None and start[2] is not None and len(start[2]) > 0)
     check_resampling(config.sample, held)
     clash_radius, clash_strength = sample_clash_guidance(config.sample)
+    connect_radius, connect_length, connect_strength = sample_connect_guidance(config.sample)
     seed_all(config.sample.seed)
     model = _load_model(config, a.device)
     allowed = _allowed_classes(config, model)
@@ -272,10 +286,12 @@ def sample_for_pocket(argv):
                                       pos_only=config.sample.pos_only, center_pos_mode=config.sample.center_pos_mode,
                                       sample_num_atoms=config.sample.sample_num_atoms, fixed_ligand=fragment,
                                       time_seq=time_seq if time_path is None else None, clash_radius=clash_radius,
-                                      clash_strength=clash_strength, allowed_types=allowed, **kw)
+                                      clash_strength=clash_strength, allowed_types=allowed, connect_radius=connect_radius,
+                                      connect_length=connect_length, connect_strength=connect_strength, **kw)
     os.makedirs(a.result_path, exist_ok=True)
     shutil.copyfile(a.config, os.path.join(a.result_path, 'sample.yml'))
     result = add_allowed_classes(add_clash_guidance(build_result(data, outputs), clash_radius, clash_strength), allowed)
+    result = add_connect_guidance(result, connect_radius, connect_length, connect_strength)
     if fragment is not None:
         result['fixed_ligand_atoms'] = int(fragment[1].shape[0])
     if start is not None:

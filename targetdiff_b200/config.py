@@ -152,6 +152,35 @@ def sample_allowed_classes(sample, mode):
     return sorted(set(cl))
 
 
+def check_connect_guidance(radius, length, strength):
+    """(radius, length, strength) as floats, or ValueError unless they are a connectivity-guidance setting (DESIGN.md section 1):
+    strength finite and >= 0, 0 turning guidance off (radius and length are then ignored and returned as None); with strength > 0 a
+    finite bond radius > 0 and a bond length with 0 < length < radius, in Angstrom.  The same refusals as tdiff_set_connect_guidance.
+    ScorePosNet3D.sample_diffusion and the config keys (sample_connect_guidance) use it."""
+    if isinstance(strength, bool) or not isinstance(strength, numbers.Real):
+        raise ValueError('connect_strength must be a number, got %r' % (strength,))
+    strength = float(strength)
+    if not math.isfinite(strength) or strength < 0:
+        raise ValueError('connect_strength must be finite and >= 0 (0 turns guidance off), got %r' % strength)
+    if strength == 0:
+        return None, None, 0.0
+    for name, x in (('connect_radius', radius), ('connect_length', length)):
+        if x is None:
+            raise ValueError('connect_strength=%g needs a %s' % (strength, name))
+        if isinstance(x, bool) or not isinstance(x, numbers.Real) or not math.isfinite(float(x)) or float(x) <= 0:
+            raise ValueError('%s must be a finite number > 0 (Angstrom), got %r' % (name, x))
+    if not float(length) < float(radius):
+        raise ValueError('connect_length=%g must be below connect_radius=%g' % (float(length), float(radius)))
+    return float(radius), float(length), strength
+
+
+def sample_connect_guidance(sample):
+    """(radius, length, strength) of `sample.connect_radius`, `sample.connect_length` and `sample.connect_strength` (an extension
+    beyond the reference's sampling.yml): strength defaults to 0 (off); radius and length have no default.  check_connect_guidance's
+    refusals, as ValueError."""
+    return check_connect_guidance(sample.get('connect_radius'), sample.get('connect_length'), sample.get('connect_strength', 0.0))
+
+
 def sampling_time_path(sample, T, base, held):
     """The resampled time path of check_resampling's (r, j): sampling.resampled_time_path over `base`, the chain's decreasing time
     sequence (T - 1, ..., 0 when it is None), or None when r = 1."""

@@ -22,6 +22,7 @@
 
 #include "../../include/tdiff.h"
 #include "sampler.cuh"
+static_assert(TD_CONNECT_MAX == TDIFF_CONNECT_MAX_ATOMS, "the connectivity kernel's shared arrays hold the documented limit");
 #include "tdiff_common.cuh"
 
 static thread_local char g_err[1024] = "";
@@ -148,6 +149,10 @@ struct tdiff_engine {
   // [N] float4: the guided x0 predictions of a step at the ligand rows (clash_guidance_kernel), the epilogue's xm_final
   float clash_radius = 0.f, clash_strength = 0.f;
   DevBuf guided;
+  // connectivity guidance (tdiff_set_connect_guidance): off while connect_strength == 0; a handle setting, kept across tdiff_bind_batch.
+  // It writes the same guided rows (connect_guidance_kernel).  max_lc: the bound batch's largest ligand, checked at chain start
+  float connect_radius = 0.f, connect_length = 0.f, connect_strength = 0.f;
+  int max_lc = 0;
   // element constraints (tdiff_set_type_mask): [Nl] uint32 class bit masks, armed while has_type_mask; cleared by tdiff_bind_batch
   bool has_type_mask = false;
   DevBuf type_mask;
@@ -656,11 +661,12 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   cudaStream_t st = (cudaStream_t)stream;
   CK(cudaSetDevice(e->device));
   long long N = 0, Np = 0, Nl = 0;
-  int max_ng = 0;
+  int max_ng = 0, max_lc_all = 0;
   for (int g = 0; g < B; ++g) {
     if (pc[g] < 0 || lc[g] < 0) return set_err(TDIFF_EINVAL, "negative atom count in graph %d", g);
     Np += pc[g]; Nl += lc[g];
     if (pc[g] + lc[g] > max_ng) max_ng = pc[g] + lc[g];
+    if (lc[g] > max_lc_all) max_lc_all = lc[g];
   }
   N = Np + Nl;
   if (N <= 0) return set_err(TDIFF_EINVAL, "empty batch");
@@ -695,7 +701,7 @@ extern "C" int tdiff_bind_batch(tdiff_engine* e, int B, const int32_t* pc, const
   e->bound = false; e->has_ligand = false; e->have_graph = false; e->have_prev = false; e->cone_evals = 0;
   e->has_fixed = false; e->fix_pos_noise = nullptr; e->fix_v_uniform = nullptr; e->has_type_mask = false;
   e->start_t = -1; e->start_pos_noise = nullptr; e->start_v_uniform = nullptr;
-  e->B = B; e->N = (int)N; e->Np = (int)Np; e->Nl = (int)Nl; e->max_ng = max_ng;
+  e->B = B; e->N = (int)N; e->Np = (int)Np; e->Nl = (int)Nl; e->max_ng = max_ng; e->max_lc = max_lc_all;
   const size_t slots = (size_t)N * K;
   int bad = 0;
   bad |= e->node_ptr.ensure((B + 1) * 4) | e->prot_ptr.ensure((B + 1) * 4) | e->prot_node.ensure(Np * 4 + 4) | e->prot_graph.ensure(Np * 4 + 4);
@@ -1251,6 +1257,15 @@ void run_step(tdiff_engine* e, cudaStream_t st, const TdStepArgs& base) {
     A.mean_noise = 0;
     e->launches += 1;
   }
+  if (e->connect_strength > 0.f) {   // connectivity guidance (DESIGN.md section 1): after clash guidance, on the same guided rows
+    TdConnectArgs C;
+    C.node_ptr = e->node_ptr.as<int>(); C.prot_ptr = e->prot_ptr.as<int>(); C.guided = e->guided.as<float4>();
+    C.radius = e->connect_radius; C.length = e->connect_length; C.strength = e->connect_strength;
+    td_launch_connect_guidance(A, C, e->B, st);
+    A.xm_final = e->guided.as<float4>();
+    A.mean_noise = 0;
+    e->launches += 1;
+  }
   td_launch_step_epilogue(A, e->has_type_mask ? e->type_mask.as<uint32_t>() : nullptr, st);
   e->launches += 2;
 }
@@ -1343,6 +1358,8 @@ int sample_chain(tdiff_engine* e, const int32_t* time_seq, int num_steps, const 
   }
   if ((d_pos_noise == nullptr) != (d_v_uniform == nullptr) && !pos_only)
     return set_err(TDIFF_EINVAL, "noise tape needs both pos_noise and v_uniform (or neither for Philox)");
+  if (e->connect_strength > 0.f && e->max_lc > TDIFF_CONNECT_MAX_ATOMS)
+    return set_err(TDIFF_EINVAL, "connectivity guidance: a graph has %d ligand atoms, more than %d", e->max_lc, TDIFF_CONNECT_MAX_ATOMS);
   if (pos_only && e->has_type_mask)
     return set_err(TDIFF_EINVAL, "a type mask is set (tdiff_set_type_mask) but pos_only keeps every atom type: clear the mask, or sample types");
   if (e->has_fixed) {      // one noise source per chain: both tapes or neither
@@ -1491,6 +1508,21 @@ extern "C" int tdiff_set_clash_guidance(tdiff_engine* e, float radius, float str
     return set_err(TDIFF_EINVAL, "set_clash_guidance: radius=%g must be finite and > 0 when strength > 0", (double)radius);
   e->clash_strength = strength;
   e->clash_radius = strength > 0.f ? radius : 0.f;
+  return TDIFF_OK;
+}
+
+extern "C" int tdiff_set_connect_guidance(tdiff_engine* e, float radius, float bond_length, float strength) {
+  if (!e) return set_err(TDIFF_EINVAL, "set_connect_guidance: null engine");
+  if (!isfinite(strength) || strength < 0.f)
+    return set_err(TDIFF_EINVAL, "set_connect_guidance: strength=%g must be finite and >= 0 (0 turns guidance off)", (double)strength);
+  if (strength > 0.f && !(isfinite(radius) && radius > 0.f))
+    return set_err(TDIFF_EINVAL, "set_connect_guidance: radius=%g must be finite and > 0 when strength > 0", (double)radius);
+  if (strength > 0.f && !(isfinite(bond_length) && bond_length > 0.f && bond_length < radius))
+    return set_err(TDIFF_EINVAL, "set_connect_guidance: bond_length=%g must be finite, > 0 and < radius=%g when strength > 0",
+                   (double)bond_length, (double)radius);
+  e->connect_strength = strength;
+  e->connect_radius = strength > 0.f ? radius : 0.f;
+  e->connect_length = strength > 0.f ? bond_length : 0.f;
   return TDIFF_OK;
 }
 

@@ -370,6 +370,110 @@ void td_launch_clash_guidance(const TdStepArgs& A, const TdGuideArgs& G, int n_g
   if (A.n_lig > 0 && n_graphs > 0) clash_guidance_kernel<<<n_graphs, TD_GUIDE_WARPS * 32, 0, st>>>(A, G);
 }
 
+// ---------------------------------------------------------------------------------------- connectivity guidance
+// Connectivity guidance (DESIGN.md section 1), before the epilogue of a denoising step and after clash guidance when both are on.  Graph
+// g's ligand rows i = 0 .. n-1 (within-graph indices) sit at q_i: the held row's target x0_f (fix_pos) when fix_mask marks it, the
+// step's x0 prediction y_i (td_pred_x0) otherwise.  Rows i, j are bonded when |q_i - q_j| < radius.  With one component every row keeps
+// y.  Otherwise each component C without a held row takes its closest outside pair (i in C, j not in C, smallest d, then lowest (i, j))
+// and moves rigidly: every row a of C gets y_a + f (q_j - q_i), f = (strength * w * (d - length)) / d, w = 1 when j's component holds a
+// held row and 1/2 otherwise; components with a held row keep y.  Every distance, comparison and the shift are explicitly rounded fp32
+// operations (no contraction), so a float32 restatement makes the same decisions, and every decision reads the graph's own rows only.
+// One CTA per graph, rows in shared memory; components by hook-and-compress union-find (roots end as the lowest index of their
+// component); the closest pair of each component as a 64-bit atomicMin key (d^2 bits << 32 | i << 16 | j).  Writes row lig_node[a] of
+// C.guided for every ligand row, held rows included (the epilogue overwrites those as before).
+#define TD_CONNECT_THREADS 256
+__device__ __forceinline__ float connect_dist2(const float* sx, const float* sy, const float* sz, int i, int j) {
+  const float dx = __fsub_rn(sx[j], sx[i]), dy = __fsub_rn(sy[j], sy[i]), dz = __fsub_rn(sz[j], sz[i]);
+  return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+}
+__global__ void __launch_bounds__(TD_CONNECT_THREADS) connect_guidance_kernel(TdStepArgs A, TdConnectArgs C) {
+  __shared__ float sx[TD_CONNECT_MAX], sy[TD_CONNECT_MAX], sz[TD_CONNECT_MAX];
+  __shared__ int par[TD_CONNECT_MAX];
+  __shared__ unsigned long long key[TD_CONNECT_MAX];
+  __shared__ unsigned char row_held[TD_CONNECT_MAX], comp_held[TD_CONNECT_MAX];
+  __shared__ int changed, n_comp;
+  const int g = blockIdx.x, tid = threadIdx.x;
+  const int lb = C.node_ptr[g] - C.prot_ptr[g], n = C.node_ptr[g + 1] - C.prot_ptr[g + 1] - lb;
+  const int s = *A.step;
+  const int t = A.seq_t ? A.seq_t[s] : A.t_start - s;
+  // the engine refuses a chain with more than TD_CONNECT_MAX ligand atoms in a graph; a graph of one atom is one component
+  const bool multi_possible = n >= 2 && n <= TD_CONNECT_MAX;
+  if (multi_possible) {
+    for (int i = tid; i < n; i += blockDim.x) {
+      const int a = lb + i;
+      const bool h = A.fix_mask && A.fix_mask[a];
+      const float4 q = h ? A.fix_pos[a] : td_pred_x0(A, a, t, A.lig_pos[a]);
+      sx[i] = q.x; sy[i] = q.y; sz[i] = q.z;
+      par[i] = i; key[i] = ~0ull; row_held[i] = h; comp_held[i] = 0;
+    }
+    if (tid == 0) { changed = 0; n_comp = 0; }
+    __syncthreads();
+    const float rho = C.radius;
+    volatile int* vp = par;
+    for (;;) {
+      // hook: for every bonded pair in different trees, the higher root points to the lower one.  Parents only decrease and always
+      // point within a component; a hook lost to a concurrent one leaves `changed` set, so the pair is seen again next round
+      for (int k = tid; k < n * n; k += blockDim.x) {
+        const int i = k / n, j = k - i * n;
+        if (j <= i || !(__fsqrt_rn(connect_dist2(sx, sy, sz, i, j)) < rho)) continue;
+        int ri = i, rj = j;
+        while (vp[ri] != ri) ri = vp[ri];
+        while (vp[rj] != rj) rj = vp[rj];
+        if (ri != rj) {
+          atomicMin(&par[max(ri, rj)], min(ri, rj));
+          changed = 1;
+        }
+      }
+      __syncthreads();
+      const bool again = changed;
+      // compress: every row points at its root
+      for (int i = tid; i < n; i += blockDim.x) {
+        int r = vp[i];
+        while (vp[r] != r) r = vp[r];
+        vp[i] = r;
+      }
+      __syncthreads();
+      if (!again) break;
+      if (tid == 0) changed = 0;
+      __syncthreads();
+    }
+    for (int i = tid; i < n; i += blockDim.x) {
+      if (row_held[i]) comp_held[par[i]] = 1;
+      if (par[i] == i) atomicAdd(&n_comp, 1);
+    }
+    __syncthreads();
+    if (n_comp > 1) {
+      for (int k = tid; k < n * n; k += blockDim.x) {
+        const int i = k / n, j = k - i * n;
+        if (par[i] == par[j]) continue;
+        const float d2 = connect_dist2(sx, sy, sz, i, j);
+        atomicMin(&key[par[i]], ((unsigned long long)__float_as_uint(d2) << 32) | ((unsigned)i << 16) | (unsigned)j);
+      }
+      __syncthreads();
+    }
+  }
+  const bool shift = multi_possible && n_comp > 1;
+  const float lam = C.strength, bl = C.length;
+  for (int i = tid; i < n; i += blockDim.x) {
+    const int a = lb + i;
+    float4 y = td_pred_x0(A, a, t, A.lig_pos[a]);
+    if (shift && !comp_held[par[i]]) {
+      const unsigned long long k = key[par[i]];
+      const int ci = (int)((k >> 16) & 0xffffu), cj = (int)(k & 0xffffu);
+      const float d = __fsqrt_rn(__uint_as_float((unsigned)(k >> 32)));
+      const float w = comp_held[par[cj]] ? 1.0f : 0.5f;
+      const float f = __fdiv_rn(__fmul_rn(__fmul_rn(lam, w), __fsub_rn(d, bl)), d);
+      y.x = __fadd_rn(y.x, __fmul_rn(f, __fsub_rn(sx[cj], sx[ci])));
+      y.y = __fadd_rn(y.y, __fmul_rn(f, __fsub_rn(sy[cj], sy[ci])));
+      y.z = __fadd_rn(y.z, __fmul_rn(f, __fsub_rn(sz[cj], sz[ci])));
+    }
+    C.guided[A.lig_node[a]] = y;
+  }
+}
+void td_launch_connect_guidance(const TdStepArgs& A, const TdConnectArgs& C, int n_graphs, cudaStream_t st) {
+  if (A.n_lig > 0 && n_graphs > 0) connect_guidance_kernel<<<n_graphs, TD_CONNECT_THREADS, 0, st>>>(A, C);
+}
+
 // Re-noising step s of a time path (tdiff_sample_path, DESIGN.md section 1): the state moves up from t = seq_t[s] to p = seq_p[s] > t
 // with the forward process, no network.  The step tables hold c = sqrt(abar_p / abar_t) in seq_c0, d = sqrt(1 - abar_p / abar_t) in
 // seq_ct, lambda = log of the type schedule's transition probability t -> p in seq_la and log(1 - e^lambda + 1e-40) in seq_l1ma.  A row

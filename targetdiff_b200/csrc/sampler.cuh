@@ -75,10 +75,21 @@ struct TdGuideArgs {
   float radius, strength;          // rho > 0 (A), lambda > 0
 };
 
+// connectivity guidance (DESIGN.md section 1): the batch layout, the bond radius, bond length and strength, and the guided x0
+// predictions.  The kernel reads each row's prediction through td_pred_x0 of its TdStepArgs, so after clash guidance (xm_final =
+// guided, mean_noise = 0) it reads and rewrites the guided rows in place
+#define TD_CONNECT_MAX 1024        // ligand atoms per graph (TDIFF_CONNECT_MAX_ATOMS): within-graph indices fit the key's 16-bit fields
+struct TdConnectArgs {
+  const int *node_ptr, *prot_ptr;  // [B+1]: graph g's ligand rows are node_ptr[g] - prot_ptr[g] .. node_ptr[g+1] - prot_ptr[g+1] - 1
+  float4* guided;                  // out [N], node-indexed: row lig_node[a] <- the guided x0 prediction of ligand row a
+  float radius, length, strength;  // rho > 0, 0 < b < rho (A), lambda > 0
+};
+
 // allowed: [Nl] class bit masks of the element constraint (tdiff_set_type_mask), or NULL for the unconstrained step
 void td_launch_step_epilogue(const TdStepArgs& A, const uint32_t* allowed, cudaStream_t st);
 void td_launch_check_type_mask(const uint32_t* allowed, int n, int n_classes, int* err, cudaStream_t st);
 void td_launch_clash_guidance(const TdStepArgs& A, const TdGuideArgs& G, int n_graphs, cudaStream_t st);
+void td_launch_connect_guidance(const TdStepArgs& A, const TdConnectArgs& C, int n_graphs, cudaStream_t st);
 void td_launch_renoise(const TdStepArgs& A, cudaStream_t st);
 void td_launch_fixed_init(const TdStepArgs& A, cudaStream_t st);
 void td_launch_start_init(const TdStepArgs& A, cudaStream_t st);

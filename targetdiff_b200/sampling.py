@@ -53,7 +53,7 @@ import numpy as np
 import torch
 
 from . import atom_num
-from .config import check_clash_guidance
+from .config import check_clash_guidance, check_connect_guidance
 from .score_model import check_time_path, check_time_seq, log_sample_categorical
 
 
@@ -191,10 +191,11 @@ def _split(arr, cum, n_data):
 def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cuda:0', num_steps=None, pos_only=False,
                             center_pos_mode='protein', sample_num_atoms='prior', rng='device', fixed_ligand=None, time_seq=None,
                             start_ligand=None, start_time=None, keep_atoms=None, time_path=None, clash_radius=None, clash_strength=0.0,
-                            allowed_types=None):
+                            allowed_types=None, connect_radius=None, connect_length=None, connect_strength=0.0):
     if rng not in ('device', 'cpu'):
         raise ValueError("rng must be 'device' or 'cpu'")
     clash_radius, clash_strength = check_clash_guidance(clash_radius, clash_strength)     # draws nothing: rng='cpu' order unchanged
+    connect = check_connect_guidance(connect_radius, connect_length, connect_strength)    # nor does connectivity guidance
     start = _check_start(model, start_ligand, start_time, keep_atoms, fixed_ligand)
     allowed = _check_allowed(allowed_types, model.num_classes, start, pos_only)          # draws nothing either
     if time_path is not None:
@@ -262,6 +263,8 @@ def sample_diffusion_ligand(model, data, num_samples, batch_size=16, device='cud
                 extra['time_path'] = time_path
             if clash_strength > 0:                                      # off is sample_diffusion's default
                 extra.update(clash_radius=clash_radius, clash_strength=clash_strength)
+            if connect[2] > 0:
+                extra.update(connect_radius=connect[0], connect_length=connect[1], connect_strength=connect[2])
             if start is not None:                                       # the clean start ligand; the engine noises it to t0
                 init_ligand_pos = start[0].to(device).repeat(n_data, 1)
                 init_ligand_v = start[1].to(device).repeat(n_data)

@@ -17,7 +17,7 @@ import torch.nn.functional as F
 import torch.nn as nn
 
 from . import _lib
-from .config import Config, check_clash_guidance, check_supported
+from .config import Config, check_clash_guidance, check_connect_guidance, check_supported
 
 GAUSSIAN_OFFSETS = (0, 1, 1.25, 1.5, 1.75, 2, 2.25, 2.5, 2.75, 3, 3.5, 4, 4.5, 5, 5.5, 6, 7, 8, 9, 10)   # models/common.py:15
 
@@ -413,7 +413,8 @@ class ScorePosNet3D(nn.Module):
     def sample_diffusion(self, protein_pos, protein_v, batch_protein, init_ligand_pos, init_ligand_v, batch_ligand,
                          num_steps=None, center_pos_mode=None, pos_only=False, noise_tape=None, seed=None, return_traj=True,
                          stack_traj=False, fixed_mask=None, fixed_noise_tape=None, time_seq=None, start_time=None, start_noise_tape=None,
-                         time_path=None, clash_radius=None, clash_strength=0.0, allowed_types=None):
+                         time_path=None, clash_radius=None, clash_strength=0.0, allowed_types=None, connect_radius=None,
+                         connect_length=None, connect_strength=0.0):
         """The reverse-diffusion chain (reference models/molopt_score_model.py:633-703), executed entirely by libtdiff.so.
 
         Extensions over the reference signature (all optional): `noise_tape=(pos_noise [S,Nl,3], v_uniform [S,Nl,K])`
@@ -456,9 +457,17 @@ class ScorePosNet3D(nn.Module):
         that ends at t = 0 ends in an allowed class; intermediate states, and the last state of a chain that stops before t = 0, are
         not restricted.  Fixed rows are held as without it (give them every class).  v0_traj / vt_traj hold -inf at forbidden
         entries where those are their values.  Not with pos_only.  Every call sets or clears the engine's mask.  No random numbers
-        are drawn.  Whether constrained molecules are chemically sensible is not measured."""
+        are drawn.  Whether constrained molecules are chemically sensible is not measured.
+
+        Connectivity guidance (DESIGN.md section 1): with `connect_strength` = lambda > 0, `connect_radius` = rho and `connect_length`
+        = b (0 < b < rho), every denoising step, after clash guidance, pulls the separate pieces of each graph's predicted ligand
+        together: atoms closer than rho are bonded (fixed rows at their targets), and each component without a fixed row moves rigidly
+        by lambda * w * (d - b) along its closest outside pair (d its length; w = 1 towards a component with a fixed row, 1/2
+        otherwise).  A graph in one piece keeps its prediction bit for bit.  At most 1024 ligand atoms per graph while it is on.  Every
+        call sets the engine's setting, off included.  No random numbers are drawn.  Whether it improves molecules is not measured."""
         T = self.num_timesteps
         clash_radius, clash_strength = check_clash_guidance(clash_radius, clash_strength)
+        connect_radius, connect_length, connect_strength = check_connect_guidance(connect_radius, connect_length, connect_strength)
         if allowed_types is not None and pos_only:
             raise ValueError('allowed_types constrains atom types, which pos_only=True keeps as they are')
         if time_path is not None:
@@ -493,6 +502,8 @@ class ScorePosNet3D(nn.Module):
         lib = _lib.load()
         st = self._stream(dev)
         _lib.check(lib.tdiff_set_clash_guidance(eng, ctypes.c_float(clash_radius or 0.0), ctypes.c_float(clash_strength)))
+        _lib.check(lib.tdiff_set_connect_guidance(eng, ctypes.c_float(connect_radius or 0.0), ctypes.c_float(connect_length or 0.0),
+                                                  ctypes.c_float(connect_strength)))
         B, Np, Nl = self._bind(eng, protein_pos, protein_v, batch_protein, batch_ligand, mode)
         lpos = init_ligand_pos.detach().to(torch.float32).contiguous()
         lv = init_ligand_v.detach().to(torch.int64).contiguous()
